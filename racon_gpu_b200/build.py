@@ -31,10 +31,16 @@ def _nvcc() -> str:
     raise RuntimeError("nvcc not found: the POA engine has no CPU fallback")
 
 
-def needs_build() -> bool:
-    if not os.path.exists(LIB):
+#: test build: every DP fill hashed per sequence (poa_core.cuh POA_FILL_DIGEST, b200poa_debug_fill_digest), so that the
+#: CUDA fill can be compared with its scalar twin in tests/emu.  Same sources and flags as the product plus one define.
+DIGEST_LIB = os.path.join(HERE, "variants", "libb200poa_digest.so")
+DIGEST_FLAGS = ["-DPOA_FILL_DIGEST=1"]
+
+
+def needs_build(lib: str = LIB) -> bool:
+    if not os.path.exists(lib):
         return True
-    t = os.path.getmtime(LIB)
+    t = os.path.getmtime(lib)
     for f in SOURCES + HEADERS:
         path = os.path.join(CSRC, f)
         if os.path.exists(path) and os.path.getmtime(path) > t:
@@ -42,23 +48,26 @@ def needs_build() -> bool:
     return False
 
 
-def build(force: bool = False, verbose: bool = False) -> str:
-    if not force and not needs_build():
-        return LIB
+def build(force: bool = False, verbose: bool = False, digest: bool = False) -> str:
+    """Build the product library, or with digest=True the test build DIGEST_LIB."""
+    lib, extra = (DIGEST_LIB, DIGEST_FLAGS) if digest else (LIB, [])
+    if not force and not needs_build(lib):
+        return lib
+    os.makedirs(os.path.dirname(lib), exist_ok=True)
     srcs = [os.path.join(CSRC, f) for f in SOURCES if os.path.exists(os.path.join(CSRC, f))]
-    cmd = [_nvcc(), *NVCC_FLAGS, "-x", "cu", "-I", os.path.join(HERE, "..", "include"), "-I", CSRC,
-           "-o", LIB, *srcs]
+    cmd = [_nvcc(), *NVCC_FLAGS, *extra, "-x", "cu", "-I", os.path.join(HERE, "..", "include"), "-I", CSRC,
+           "-o", lib, *srcs]
     res = subprocess.run(cmd, capture_output=True, text=True)
     log = res.stdout + res.stderr
-    with open(os.path.join(HERE, "build.log"), "w") as fh:
+    with open(os.path.join(HERE, "build.log") if not digest else lib[:-3] + ".build.log", "w") as fh:
         fh.write(" ".join(cmd) + "\n" + log)
     if res.returncode != 0:
         sys.stderr.write(log)
-        raise RuntimeError("nvcc failed building libb200poa.so")
+        raise RuntimeError(f"nvcc failed building {os.path.basename(lib)}")
     if verbose:
         print(log)
-    return LIB
+    return lib
 
 
 if __name__ == "__main__":
-    print(build(force="--force" in sys.argv, verbose=True))
+    print(build(force="--force" in sys.argv, verbose=True, digest="--digest" in sys.argv))

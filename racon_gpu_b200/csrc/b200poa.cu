@@ -68,6 +68,10 @@ struct KernelArgs {
     int32_t ring_stride; /* int16 cells per ring row     */
     int32_t ring_rows;   /* power of two                 */
     unsigned long long* phase_cycles; /* diagnostics: [PH_COUNT] or nullptr */
+#if POA_FILL_DIGEST
+    unsigned long long* fill_digest; /* [staged sequences] see b200poa_debug_fill_digest */
+    int32_t* fill_count;
+#endif
 };
 
 #ifndef POA_MIN_BLOCKS_PER_SM
@@ -121,6 +125,10 @@ __global__ void __launch_bounds__(32, POA_MIN_BLOCKS_PER_SM) poa_window_kernel(c
         wv.seq_begin = a.seq_begin + s0;
         wv.seq_end = a.seq_end + s0;
         wv.path = a.path;
+#if POA_FILL_DIGEST
+        wv.fill_digest = a.fill_digest + s0;
+        wv.fill_count = a.fill_count + s0;
+#endif
         WindowOut out;
         out.cons = a.out_cons;
         out.cov = a.out_cov;
@@ -250,6 +258,10 @@ struct b200poa_batch {
     int32_t* h_msa_cols = nullptr;
     int32_t* h_msa_status = nullptr;
     int32_t* h_msa_rows = nullptr;         /* sequences staged per window = rows of its MSA */
+#if POA_FILL_DIGEST
+    unsigned long long* d_fill_digest = nullptr; /* [max_seqs] per staged sequence, see b200poa_debug_fill_digest */
+    int32_t* d_fill_count = nullptr;
+#endif
     size_t msa_cap = 0;
     size_t msa_bound = 0;                  /* worst-case MSA bytes of the windows staged so far */
     bool msa_fetched = false;
@@ -288,10 +300,11 @@ static SmemGeometry smem_geometry(const Params& p, int32_t max_len) {
      * [l*8*NV, (l+1)*8*NV): lanes past the read still load -- never store -- profile bytes and ring cells up to
      * column 256*NV.  Rows are therefore sized by the longest read only, and the allocation ends with enough slack
      * for the loads of the last row. */
-    const int32_t nv = (colsP + 255) / 256;
     g.prof_stride = banded ? std::max(colsP, 256) : colsP;
     const int32_t row_cells = banded ? std::max(p.band_width, 256) : colsP;
-    const int32_t slack_cells = banded ? 0 : 256 * nv - colsP;
+    /* in a banded batch the reads shorter than the band take fill_rows_wide too: a band of 384 columns runs reads of up
+     * to 384 columns with NV = 2, whose lanes load up to column 512 of the last ring row */
+    const int32_t slack_cells = 256 * ((row_cells + 255) / 256) - row_cells;
     g.ring_stride = row_cells + RING_PAD_FRONT + RING_PAD_BACK;
     int32_t ring_bytes = 4096;
     {   /* at least 8 ring rows: a predecessor more than 7 ranks back is rare (0.6%), more than 3 is not (19%) */
@@ -361,6 +374,10 @@ static void free_batch(b200poa_batch* b) {
     cudaFreeHost(b->h_msa_cols);
     cudaFreeHost(b->h_msa_status);
     cudaFreeHost(b->h_msa_rows);
+#if POA_FILL_DIGEST
+    cudaFree(b->d_fill_digest);
+    cudaFree(b->d_fill_count);
+#endif
     delete b;
 }
 
@@ -558,6 +575,10 @@ static int32_t alloc_batch_memory(b200poa_batch* b) {
     CU_TRY(cudaHostAlloc(&b->h_out_off, MP * sizeof(int32_t), cudaHostAllocDefault));
     CU_TRY(cudaHostAlloc(&b->h_trim, MP * sizeof(int32_t), cudaHostAllocDefault));
     CU_TRY(cudaHostAlloc(&b->h_cursor, 2 * sizeof(int32_t), cudaHostAllocDefault));
+#if POA_FILL_DIGEST
+    CU_TRY(cudaMalloc(&b->d_fill_digest, (MS + 1) * sizeof(unsigned long long)));
+    CU_TRY(cudaMalloc(&b->d_fill_count, (MS + 1) * sizeof(int32_t)));
+#endif
     return B200POA_SUCCESS;
 }
 
@@ -940,6 +961,12 @@ int32_t b200poa_batch_launch(b200poa_batch* b) {
     a.p.ring_rows = b->ring_rows;
     a.p.ring_stride = b->ring_stride;
     a.phase_cycles = b->d_phase;
+#if POA_FILL_DIGEST
+    CU_TRY(cudaMemsetAsync(b->d_fill_digest, 0, (size_t)b->seq_count * sizeof(unsigned long long), b->stream));
+    CU_TRY(cudaMemsetAsync(b->d_fill_count, 0, (size_t)b->seq_count * sizeof(int32_t), b->stream));
+    a.fill_digest = b->d_fill_digest;
+    a.fill_count = b->d_fill_count;
+#endif
     /* persistent grid: one warp per resident slot.  (Shrinking the grid so that every round of it is full --
      * 10000 windows as 3 x 3334 instead of 2.8 x 3552 -- was measured neutral: throughput follows the number of
      * resident warps.  B200POA_GRID_BALANCE=1 keeps the experiment available.) */
@@ -1109,6 +1136,23 @@ int32_t b200poa_batch_get_info(const b200poa_batch* b, b200poa_batch_info* info)
 }
 
 } // extern "C"
+
+#if POA_FILL_DIGEST
+/* test build only (not part of include/b200poa.h): after the last launch, per staged sequence (staging order: windows in
+ * add order, each window's sequences in processing order) the sum of the digests of its DP fills and their number, and
+ * the score-row ring the launch used.  Synchronises. */
+extern "C" int32_t b200poa_debug_fill_digest(b200poa_batch* b, uint64_t* digest, int32_t* count, int64_t n,
+                                             int32_t* ring_rows, int32_t* ring_stride) {
+    if (!b || !digest || !count || n < b->seq_count) return B200POA_INVALID_ARGUMENT;
+    DeviceGuard g(b->device);
+    CU_TRY(cudaStreamSynchronize(b->stream));
+    CU_TRY(cudaMemcpy(digest, b->d_fill_digest, (size_t)b->seq_count * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+    CU_TRY(cudaMemcpy(count, b->d_fill_count, (size_t)b->seq_count * sizeof(int32_t), cudaMemcpyDeviceToHost));
+    if (ring_rows) *ring_rows = b->ring_rows;
+    if (ring_stride) *ring_stride = b->ring_stride;
+    return B200POA_SUCCESS;
+}
+#endif
 
 #if defined(B200POA_SUBTIMERS)
 /* experiments only (not part of include/b200poa.h): sub-phase cycle counters since the last call */

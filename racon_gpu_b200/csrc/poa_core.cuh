@@ -40,6 +40,12 @@
 #pragma once
 #include "poa_simt.cuh"
 
+/* Test build (-DPOA_FILL_DIGEST=1, racon_gpu_b200/variants/libb200poa_digest.so and tests/emu): every DP fill is hashed
+ * (fill_digest) so that the CUDA fill can be compared cell for cell with its scalar twin.  The product never has it. */
+#ifndef POA_FILL_DIGEST
+#define POA_FILL_DIGEST 0
+#endif
+
 namespace b200poa {
 
 POA_FN void poa_atomic_add(uint32_t* p, uint32_t v) {
@@ -239,6 +245,10 @@ struct WindowView {
                                  every base of every sequence was assigned to -- the sequence's path through the graph,
                                  which spoa re-derives from edge labels (Node::successor, graph.cpp:31-43) and cudapoa
                                  from per-edge sequence lists (outgoing_edges_coverage, cudapoa_add_alignment.cuh:245-262) */
+#if POA_FILL_DIGEST
+    unsigned long long* fill_digest; /* [n_seqs] test build only: sum of fill_digest() over every fill of the sequence */
+    int32_t* fill_count;             /* [n_seqs] fills of the sequence (adaptive retries included) */
+#endif
 };
 
 /* Where a window's result goes: consensus and coverage are appended to compact arenas (one bump allocation per
@@ -478,6 +488,41 @@ POA_FN ReadGeom read_geometry(const Params& p, int32_t len, int32_t n_rows, int3
     g.bw = g.banded ? band_width : g.colsP;
     g.step = ((uint32_t)len << 16) / (uint32_t)(n_rows > 0 ? n_rows : 1); /* len < 2^15 by the config limits */
     return g;
+}
+
+/* Which DP fill a read on int16 cells takes (poa_fill.cuh, CudaFill); a read on 32-bit cells always runs fill_rows_i32.
+ * One rule for the kernel and the emulation, which reports per window how many reads took each variant. */
+enum FillVariant : int32_t {
+    FILL_WIDE1 = 0,      /* full band, colsP <= 256: fill_rows_wide<1> ... */
+    FILL_WIDE2,          /* ... <= 512 */
+    FILL_WIDE3,          /* ... <= 768 */
+    FILL_WIDE4,          /* ... <= 1024: fill_rows_wide<4> */
+    FILL_CHUNKED_FULL,   /* full band over more than 1024 columns: fill_rows<false>, 256-column chunk passes */
+    FILL_FULLW,          /* static band of exactly 256 columns: fill_rows<true> */
+    FILL_CHUNKED_BANDED, /* any other band width: fill_rows<false> */
+    FILL_VARIANTS
+};
+/* The rule, written once: calls visitor.run<variant>() for the variant of a read.  CudaFill runs the fill itself
+ * through it (the same branches as a plain if-chain, so the kernel's code does not depend on this indirection). */
+#if POA_DEVICE
+#pragma nv_exec_check_disable
+#endif
+template <class Visitor>
+POA_HD int32_t fill_dispatch(const ReadGeom& g, Visitor& v) {
+    if (g.banded) return (g.bw == CHUNK) ? v.template run<FILL_FULLW>() : v.template run<FILL_CHUNKED_BANDED>();
+    if (g.colsP <= 256) return v.template run<FILL_WIDE1>();
+    if (g.colsP <= 512) return v.template run<FILL_WIDE2>();
+    if (g.colsP <= 768) return v.template run<FILL_WIDE3>();
+    if (g.colsP <= 1024) return v.template run<FILL_WIDE4>();
+    return v.template run<FILL_CHUNKED_FULL>();
+}
+struct FillVariantOf {
+    template <int32_t V>
+    POA_HD int32_t run() { return V; }
+};
+POA_HD int32_t fill_variant(const ReadGeom& g) {
+    FillVariantOf v;
+    return fill_dispatch(g, v);
 }
 
 /* Copies of the geometry / parameters a phase function received by reference (i.e. through local memory, which
@@ -2660,6 +2705,49 @@ POA_HD bool score_range_ok(const Params& p, int32_t n_columns, int32_t len) {
     return lo > NEG + 512 && hi < 32000;
 }
 
+#if POA_FILL_DIGEST
+POA_FN unsigned long long digest_mix64(unsigned long long x) { /* splitmix64's finaliser */
+    x ^= x >> 30;
+    x *= 0xbf58476d1ce4e5b9ull;
+    x ^= x >> 27;
+    x *= 0x94d049bb133111ebull;
+    x ^= x >> 31;
+    return x;
+}
+/* Hash of the score rows the fill of one read just wrote: the wrapping sum, over the real cells (rows 1..n_rows, columns
+ * [band start, band start + bw) within [0, len]), of mix64(row, column, value).  A sum does not depend on the order in
+ * which lanes visit cells.  Cells past the read are not specified by the fill's contract and are not hashed. */
+POA_FN_NOINLINE unsigned long long fill_digest(const Slot& s_ref, const Params p, const ReadGeom g_ref, int32_t cells32) {
+    const Slot s = s_ref;
+    const ReadGeom g = geom_uniform(g_ref);
+    const int32_t* const S32 = reinterpret_cast<const int32_t*>(s.S);
+    PerLane<unsigned long long> acc;
+    POA_LANES(l) { acc[l] = 0; }
+    for (int32_t i = 1; i <= g.n_rows; ++i) {
+        const int32_t bs = rec_bs(s.row_rec[i]);
+        const size_t row = (size_t)i * (size_t)p.stride;
+        POA_LANES(l) {
+            for (int32_t o = l; o < g.bw && bs + o <= g.len; o += 32) {
+                const int32_t v = cells32 ? S32[row + o] : (int32_t)s.S[row + o];
+                const unsigned long long key = (unsigned long long)(uint32_t)v | ((unsigned long long)(bs + o) << 32) |
+                                               ((unsigned long long)i << 48);
+                acc[l] += digest_mix64(key + 0x9e3779b97f4a7c15ull);
+            }
+        }
+    }
+#if POA_DEVICE
+    unsigned long long t = acc[0];
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) t += __shfl_xor_sync(0xffffffffu, t, d);
+    return t;
+#else
+    unsigned long long t = 0;
+    for (int l = 0; l < 32; ++l) t += acc[l];
+    return t;
+#endif
+}
+#endif
+
 /* ------------------------------------------------------------------------------------------
  * One window, start to finish  (racon::Window::generate_consensus, src/window.cpp:65-116, for
  * full-span layers; the caller trims).  Fill is the DP-fill functor:
@@ -2764,6 +2852,16 @@ POA_FN int32_t process_window(const Slot& s, const Params& p, const WindowView& 
             if (st.status != ST_SUCCESS) break;
             const int32_t end_row = poa_uniform(cells32 ? fill_rows_i32(s, p, g, read) : fill(s, p, st, g, read));
             POA_FENCE(); /* the score rows must be in place before the traceback's asynchronous copies read them */
+#if POA_FILL_DIGEST
+            {
+                const unsigned long long d = fill_digest(s, p, g, cells32 ? 1 : 0);
+                POA_LANE0 {
+                    wv.fill_digest[r] += d;
+                    wv.fill_count[r] += 1;
+                }
+                POA_SYNC();
+            }
+#endif
             tm.lap(PH_FILL);
             st.band_hit = 0;
 #if POA_DEVICE && POA_PREFETCH_GRAPH && POA_PREFETCH_GRAPH != 3

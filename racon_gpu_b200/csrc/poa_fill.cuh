@@ -633,13 +633,21 @@ struct CudaFill {
         fa.mg = p.match - p.gap;
         fa.xg = p.mismatch - p.gap;
         fa.gap = p.gap;
-        if (g.banded) return (g.bw == CHUNK) ? fill_rows<true>(fa) : fill_rows<false>(fa);
-        if (g.colsP <= 256) return fill_rows_wide<1>(fa);
-        if (g.colsP <= 512) return fill_rows_wide<2>(fa);
-        if (g.colsP <= 768) return fill_rows_wide<3>(fa);
-        if (g.colsP <= 1024) return fill_rows_wide<4>(fa);
-        return fill_rows<false>(fa); /* longer reads: 256-column chunk passes */
+        Run run{fa};
+        return fill_dispatch(g, run); /* fill_variant()'s rule */
     }
+    struct Run {
+        const FillArgs& fa;
+        template <int32_t V>
+        __device__ __forceinline__ int32_t run() {
+            if (V == FILL_FULLW) return fill_rows<true>(fa);
+            if (V == FILL_WIDE1) return fill_rows_wide<1>(fa);
+            if (V == FILL_WIDE2) return fill_rows_wide<2>(fa);
+            if (V == FILL_WIDE3) return fill_rows_wide<3>(fa);
+            if (V == FILL_WIDE4) return fill_rows_wide<4>(fa);
+            return fill_rows<false>(fa); /* FILL_CHUNKED_BANDED (other band widths), FILL_CHUNKED_FULL (256-column passes) */
+        }
+    };
 };
 
 #endif /* POA_DEVICE */

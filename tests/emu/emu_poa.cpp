@@ -22,14 +22,61 @@ using namespace b200poa;
 
 namespace {
 
+/* Reach report: per window, which paths of the CUDA fill its reads would take (tests/fill_cases.py names the fields). */
+enum Reach {
+    R_VARIANT = 0,                  /* [FILL_VARIANTS] reads per fill_variant() (int16 cells) */
+    R_CELLS32 = R_VARIANT + FILL_VARIANTS, /* fills on 32-bit cells (fill_rows_i32) */
+    R_GENERAL_ROWS,                 /* rows flagged for the general path (pred_needs_general_path) */
+    R_FAR_PREDS,                    /* predecessors older than the ring */
+    R_JUMP_PREDS,                   /* predecessors whose band starts more than RING_PAD_BACK columns before the row's */
+    R_MAX_NPRED,                    /* largest predecessor count of a row */
+    R_ROWS_OVER32,                  /* rows with more than 32 predecessors */
+    R_DYN_ROWS,                     /* rows whose letter needs the on-demand profile row */
+    R_DYN_BUILDS,                   /* times that row is (re)built: the letter changed since the last such row */
+    R_RETRIES,                      /* adaptive retries (a read filled again) */
+    R_RETRIES_FULL,                 /* ... that reached the full matrix */
+    R_MAX_LEN,                      /* longest read filled */
+    R_FIELDS
+};
+
 /* Scalar twin of poa_fill.cuh: same cell definition, same NEG clamp, same band. */
 struct ScalarFill {
     int64_t cells = 0;
+    int32_t* reach = nullptr; /* this window's report, or nullptr */
+    const uint8_t* last_read = nullptr;
     int32_t operator()(const Slot& s, const Params& p, WinState& st, const ReadGeom& g,
                        const uint8_t* read) {
         const int32_t N = g.n_rows;
         (void)st;
         const int32_t mg = p.match - p.gap, xg = p.mismatch - p.gap;
+        if (reach) {
+            reach[R_VARIANT + fill_variant(g)] += 1;
+            if (read == last_read) {
+                reach[R_RETRIES] += 1;
+                if (!g.banded) reach[R_RETRIES_FULL] += 1;
+            }
+            if (g.len > reach[R_MAX_LEN]) reach[R_MAX_LEN] = g.len;
+            int32_t dyn_code = -1;
+            for (int32_t i = 1; i <= N; ++i) {
+                const uint32_t rec = s.row_rec[i];
+                const int32_t np = rec_npred(rec), po = (int32_t)s.row_poff[i];
+                if (rec_far(rec)) reach[R_GENERAL_ROWS] += 1;
+                if (np > reach[R_MAX_NPRED]) reach[R_MAX_NPRED] = np;
+                if (np > 32) reach[R_ROWS_OVER32] += 1;
+                if (rec_prow(rec) == 4) {
+                    reach[R_DYN_ROWS] += 1;
+                    if (rec_code(rec) != dyn_code) reach[R_DYN_BUILDS] += 1;
+                    dyn_code = rec_code(rec);
+                }
+                for (int32_t k = 0; k < np; ++k) {
+                    const uint32_t pe = s.row_pred[po + k];
+                    const int32_t pr = (int32_t)(pe & 0xFFFFu), pbs = (int32_t)(pe >> 16);
+                    if (i - pr >= p.ring_rows) reach[R_FAR_PREDS] += 1;
+                    if (rec_bs(rec) - pbs > RING_PAD_BACK) reach[R_JUMP_PREDS] += 1;
+                }
+            }
+        }
+        last_read = read;
         for (int32_t c = 0; c < g.bw; ++c) s.S[c] = 0; /* row 0: H = j*gap  =>  S = 0 */
         int32_t best = NEG, end_row = 0;
         for (int32_t i = 1; i <= N; ++i) {
@@ -84,7 +131,11 @@ void emu_polish_windows(int64_t n_windows, const int64_t* win_seq_off, const int
                         uint16_t* cov_out, int32_t stride_out, int32_t* cons_len, int32_t* status,
                         int32_t* rank_out, int32_t* n_nodes_out, int64_t* cells_out, int32_t* trim_out,
                         /* MSA (all nullable): compact arena of msa_cap bytes + per-window offset / columns / status */
-                        uint8_t* msa_out, int64_t msa_cap, int64_t* msa_off, int32_t* msa_cols, int32_t* msa_status) {
+                        uint8_t* msa_out, int64_t msa_cap, int64_t* msa_off, int32_t* msa_cols, int32_t* msa_status,
+                        /* ring_rows: the score-row ring of the GPU launch to compare with (the row program's far-predecessor
+                         * flags depend on it).  Per sequence (window by window, processing order; nullable): the sum of
+                         * fill_digest() over its fills and their number.  Per window (nullable): R_FIELDS reach counters. */
+                        int32_t ring_rows, unsigned long long* digest_out, int32_t* fill_count_out, int32_t* reach_out) {
     Params p;
     p.max_nodes = max_nodes;
     p.max_edges = poa_edge_capacity(max_nodes); /* the engine derives the edge pool from the node capacity */
@@ -103,7 +154,7 @@ void emu_polish_windows(int64_t n_windows, const int64_t* win_seq_off, const int
     p.wide_cells = (p.force_cells32 || !score_range_ok(p, p.max_nodes, p.max_len)) ? 1 : 0;
     p.serial_topsort = serial_topsort & 1;
     p.skip_consensus = 0;
-    p.ring_rows = 8;
+    p.ring_rows = ring_rows;
     p.ring_stride = p.stride;
     Slot probe;
     size_t slot_bytes = 0;
@@ -181,6 +232,15 @@ void emu_polish_windows(int64_t n_windows, const int64_t* win_seq_off, const int
             wv.seq_end = wend.data();
             std::vector<uint16_t> wpath(msa_out ? wbases.size() + 1 : 0);
             wv.path = msa_out ? wpath.data() : nullptr;
+            std::vector<unsigned long long> wdigest((size_t)n, 0);
+            std::vector<int32_t> wcount((size_t)n, 0);
+            wv.fill_digest = wdigest.data();
+            wv.fill_count = wcount.data();
+            int32_t* reach = reach_out ? reach_out + w * R_FIELDS : nullptr;
+            if (reach)
+                for (int32_t k = 0; k < R_FIELDS; ++k) reach[k] = 0;
+            fill.reach = reach;
+            fill.last_read = nullptr;
             /* process_window writes its node count nowhere; recover it from the slot afterwards */
             uint32_t cursor = 0;
             int32_t off = 0, trim = 0;
@@ -196,6 +256,16 @@ void emu_polish_windows(int64_t n_windows, const int64_t* win_seq_off, const int
             long long moff = 0;
             int32_t mcols = 0, mst = 0;
             const int32_t n_final = process_window(s, p, wv, fill, tbs, out);
+            if (digest_out)
+                for (int32_t k = 0; k < n; ++k) digest_out[s0 + k] = wdigest[(size_t)k];
+            if (fill_count_out)
+                for (int32_t k = 0; k < n; ++k) fill_count_out[s0 + k] = wcount[(size_t)k];
+            if (reach) { /* fills that did not go through the int16 twin ran on 32-bit cells */
+                int32_t fills = 0, fills16 = 0;
+                for (int32_t k = 0; k < n; ++k) fills += wcount[(size_t)k];
+                for (int32_t v = 0; v < FILL_VARIANTS; ++v) fills16 += reach[R_VARIANT + v];
+                reach[R_CELLS32] = fills - fills16;
+            }
             if (msa_out) {
                 MsaOut mo;
                 mo.arena = msa_out;

@@ -11,6 +11,11 @@ from oracle_lib import _flat_args, _p
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 
+#: per-window reach counters of the emulated fill (enum Reach in tests/emu/emu_poa.cpp), in order
+REACH_FIELDS = ("wide1", "wide2", "wide3", "wide4", "chunked_full", "fullw", "chunked_banded", "cells32",
+                "general_rows", "far_preds", "jump_preds", "max_npred", "rows_over32", "dyn_rows", "dyn_builds",
+                "retries", "retries_full", "max_len")
+
 
 class Emu:
     def __init__(self):
@@ -19,8 +24,11 @@ class Emu:
         self.lib = C.CDLL(os.path.join(HERE, "emu", "libpoa_emu.so"))
 
     def polish(self, b, order, m, x, g, max_nodes=4096, max_edges=24576, max_len=1023, band=0,
-               serial_topsort=False, threads=8, stride=4096, msa_cap=0):
-        """Untrimmed consensus, coverage, status and DP cell count of the emulated engine."""
+               serial_topsort=False, threads=8, stride=4096, msa_cap=0, ring_rows=8):
+        """Untrimmed consensus, coverage, status and DP cell count of the emulated engine.  Also kept: per sequence
+        (ADD order index of the window's first sequence + processing position) the fill digest and fill count
+        (last_digest, last_fill_count), per window the reach counters (last_reach: dict REACH_FIELDS -> array).
+        ring_rows: the GPU launch's score-row ring, which decides the row program's far-predecessor flags."""
         W = b.n_windows
         cons = np.zeros((W, stride), dtype=np.uint8)
         cov = np.zeros((W, stride), dtype=np.uint16)
@@ -28,6 +36,9 @@ class Emu:
         st = np.zeros(W, dtype=np.int32)
         cells = C.c_int64(0)
         self.last_trim = np.zeros(W, dtype=np.int32)  # device-side trim interval: first | last << 16
+        self.last_digest = np.zeros(b.n_seqs, dtype=np.uint64)
+        self.last_fill_count = np.zeros(b.n_seqs, dtype=np.int32)
+        reach = np.zeros((W, len(REACH_FIELDS)), dtype=np.int32)
         order = np.ascontiguousarray(order, dtype=np.int32)
         a = _flat_args(b)
         self.lib.emu_polish_windows(
@@ -35,7 +46,9 @@ class Emu:
             C.c_int32(max_nodes), C.c_int32(max_edges), C.c_int32(max_len), C.c_int32(band),
             C.c_int32(int(serial_topsort)), C.c_int32(threads), _p(cons, C.c_uint8), _p(cov, C.c_uint16),
             C.c_int32(stride), _p(clen, C.c_int32), _p(st, C.c_int32), None, None, C.byref(cells),
-            _p(self.last_trim, C.c_int32), *self._msa_args(W, msa_cap))
+            _p(self.last_trim, C.c_int32), *self._msa_args(W, msa_cap), C.c_int32(ring_rows),
+            _p(self.last_digest, C.c_uint64), _p(self.last_fill_count, C.c_int32), _p(reach, C.c_int32))
+        self.last_reach = {k: reach[:, i].copy() for i, k in enumerate(REACH_FIELDS)}
         self.last_msa = None
         if msa_cap:  # per window: list of rows (processing order), or the status when the MSA failed
             arena, off, cols, mst = self._msa

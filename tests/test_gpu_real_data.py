@@ -28,6 +28,22 @@ def test_lambda_windows_full_band_equal_racon_cpu(oracle, case, golden, via_adap
     assert contig_edit_distance(oracle, got, lambda_reference()) == golden
 
 
+def test_lambda_w1000_windows_full_band_equal_racon_cpu(oracle):
+    """test/racon_test.cpp:180-195 (window length 1000) on the GPU with max_sequence_size 2047: the longest reads (up to
+    1155 bases) are longer than fill_rows_wide covers and take the chunked full-band fill.  Every window equals racon's
+    CPU consensus with the same polished flag, and the contig is at edit distance 1289."""
+    b, cons, polished, p = lambda_fixture("fastq_1000")
+    assert p["window_length"] == 1000 and int(np.diff(b.seq_off).max()) > 1024
+    pol = api.Polisher(devices=[0], mem_per_batch=16 << 30, max_sequence_size=2047, match=p["m"], mismatch=p["x"],
+                       gap=p["g"])
+    got_c, got_l, got_p, status = pol.polish(b, tgs=p["tgs"], trim=p["trim"], stride=4096)
+    pol.close()
+    got = api.consensus_list(got_c, got_l)
+    assert (got_p == polished).all()
+    assert got == cons
+    assert contig_edit_distance(oracle, got, lambda_reference()) == 1289
+
+
 @pytest.mark.parametrize("case,golden", [("fastq_500", 1312), ("fasta_500", 1566)])
 def test_lambda_windows_static_band_within_tolerance(oracle, case, golden):
     """Banded mode on real windows: stated tolerance vs racon's unbanded CPU consensus (>= 99 % of the windows
