@@ -47,8 +47,8 @@ static void emit(opbuf* o, uint8_t op, int64_t count) {
 }
 
 /* last column of the distance matrix of q[0..n) (step sq: +1 forward, -1 backward from q) against t[0..m) (step st):
- * col[i] = D[i][m], i = 0..n */
-static void last_column(const char* q, int32_t n, int sq, const char* t, int32_t m, int st, int32_t* col) {
+ * col[i] = D[i][m], i = 0..n.  Exported: the tests hold the engine's Hirschberg middle columns against it. */
+void aln_oracle_last_column(const char* q, int32_t n, int sq, const char* t, int32_t m, int st, int32_t* col) {
     for (int32_t i = 0; i <= n; ++i) col[i] = i;
     for (int32_t j = 1; j <= m; ++j) {
         const char tc = t[(int64_t)(j - 1) * st];
@@ -124,8 +124,8 @@ static int align_rec(const char* q, int32_t n, const char* t, int32_t m, int32_t
     const int32_t lh = m / 2, rh = m - lh; /* edlib.cpp:1216-1217 */
     int32_t* L = (int32_t*)malloc(sizeof(int32_t) * (size_t)(n + 1));
     int32_t* Rr = (int32_t*)malloc(sizeof(int32_t) * (size_t)(n + 1));
-    last_column(q, n, 1, t, lh, 1, L);                      /* L[i]  = D(q[0..i), t[0..lh))                */
-    last_column(q + n - 1, n, -1, t + m - 1, rh, -1, Rr);   /* Rr[i] = D(q[n-i..n), t[lh..m))              */
+    aln_oracle_last_column(q, n, 1, t, lh, 1, L);                      /* L[i]  = D(q[0..i), t[0..lh))                */
+    aln_oracle_last_column(q + n - 1, n, -1, t + m - 1, rh, -1, Rr);   /* Rr[i] = D(q[n-i..n), t[lh..m))              */
     int32_t r = -2, ls = 0, rs = 0;
     for (int32_t idx = 0; idx <= n - 2; ++idx) { /* edlib.cpp:1282-1290: scoresLeft[idx] + scoresRight[idx + 1] */
         if (L[idx + 1] + Rr[n - idx - 1] == best) {
@@ -158,7 +158,7 @@ static int align_rec(const char* q, int32_t n, const char* t, int32_t m, int32_t
 int64_t aln_oracle_nw(const char* q, int32_t n, const char* t, int32_t m, uint8_t* ops, int64_t cap, int32_t* score) {
     if (n <= 0 || m <= 0) return -1;
     int32_t* col = (int32_t*)malloc(sizeof(int32_t) * (size_t)(n + 1));
-    last_column(q, n, 1, t, m, 1, col);
+    aln_oracle_last_column(q, n, 1, t, m, 1, col);
     const int32_t best = col[n];
     free(col);
     if (score) *score = best;

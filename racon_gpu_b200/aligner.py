@@ -28,6 +28,22 @@ SUCCESS, UNINITIALIZED, EXCEEDED_MAX_ALIGNMENTS, EXCEEDED_MAX_LENGTH = 0, 1, 2, 
 GENERIC_ERROR, INVALID_ARGUMENT, CUDA_ERROR = 5, 6, 7
 
 
+#: one record of the test build's split log (aln_core.cuh AlnSplitRec, b200aln_debug_split_log): a Hirschberg split
+#: attempt -- the sub-problem, the band its passes got, attempt 0 or 1 (redone without a band), level, path (SPLIT_PATHS),
+#: flags (1: a team_wait gave up), the split and order-independent hashes of both middle columns
+SPLIT_REC_DTYPE = np.dtype([("aln", "<i4"), ("r0", "<i4"), ("c0", "<i4"), ("n", "<i4"), ("m", "<i4"), ("band", "<i4"),
+                            ("attempt", "<i4"), ("level", "<i4"), ("path", "<i4"), ("flags", "<i4"), ("r", "<i4"),
+                            ("ls", "<i4"), ("rs", "<i4"), ("best", "<i4"), ("pad", "<i4", (2,)), ("lc_hash", "<u8"),
+                            ("rr_hash", "<u8")])
+SPLIT_PATHS = ("warp", "team", "side")  # one warp; a team in a thin level; a team on the side stream
+SPLIT_TIMEOUT = 1
+
+
+def is_leaf(n: int, m: int) -> bool:
+    """aln_core.cuh aln_is_leaf (edlib.cpp:1135-1157): is an n x m sub-problem traced back without a split?"""
+    return n == 0 or m == 0 or 20 * ((n + 63) // 64) * m + 8 * m < 1024 * 1024
+
+
 class AlnBatchInfo(C.Structure):
     _fields_ = [("device_id", C.c_int32), ("n_slots", C.c_int32), ("levels", C.c_int32), ("kernel_launches", C.c_int32),
                 ("team_launches", C.c_int32), ("n_team_blocks", C.c_int32),
@@ -196,6 +212,25 @@ class CUDABatchAligner:
 
     def reset(self):
         self.lib.b200aln_batch_reset(self.h)
+
+    def split_log(self) -> np.ndarray:
+        """Test build only (racon_gpu_b200/variants/libb200poa_digest.so): the split log of the last align_all, one
+        SPLIT_REC_DTYPE record per split attempt.  Raises when the log overflowed."""
+        fn = getattr(self.lib, "b200aln_debug_split_log", None)
+        if fn is None:
+            raise RuntimeError("this library has no split log: load the digest build")
+        count, rec_bytes = C.c_int64(0), C.c_int32(0)
+        st = fn(self.h, None, C.c_int64(0), C.byref(count), C.byref(rec_bytes))
+        if st not in (SUCCESS, GENERIC_ERROR):
+            raise RuntimeError(f"b200aln_debug_split_log: {status_string(st)}")
+        assert rec_bytes.value == SPLIT_REC_DTYPE.itemsize, (rec_bytes.value, SPLIT_REC_DTYPE.itemsize)
+        out = np.zeros(count.value, dtype=SPLIT_REC_DTYPE)
+        st = fn(self.h, out.ctypes.data_as(C.c_void_p), C.c_int64(count.value), C.byref(count), C.byref(rec_bytes))
+        if st == GENERIC_ERROR:
+            raise RuntimeError(f"the split log overflowed: {count.value} records appended")
+        if st != SUCCESS:
+            raise RuntimeError(f"b200aln_debug_split_log: {status_string(st)}")
+        return out
 
 
 def pack_pairs(pairs):

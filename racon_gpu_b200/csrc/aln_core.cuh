@@ -247,11 +247,48 @@ POA_FN int64_t leaf_entry(int32_t b, int32_t j, int32_t B, int32_t cols) {
  * stripe's hand-over row (global memory, row s mod n) and publishes its progress -- (stripe << 32 | columns done), one
  * word of shared memory per warp -- every 32 columns; the next stripe's warp polls that word before it fetches the row's
  * next word, 16 columns ahead of their use.  Producers never wait, so the pipeline cannot deadlock.
+ *
+ * Test builds.  ALN_EMU_TEAMS (host flavour, tests/emu only): a team's warps are threads and the primitives below call
+ * the emulation's hooks (aln_emu_*): atomic progress words, a mutex / condition-variable barrier, and a protocol checker
+ * -- every hand-over word carries a shadow tag (pass, stripe) of its writer, and every load names the stripe that must
+ * have written it and the columns the consumer's last team_wait must cover.  ALN_SPLIT_DIGEST (device test build): a
+ * team_wait gives up after ALN_WAIT_POLLS polls and flags it, so that a protocol error is a failed record, not a hung
+ * block.  Neither changes the product's code: the extra arguments are ignored there.
  * ---------------------------------------------------------------------------------------- */
+#ifndef ALN_TEAM
+#define ALN_TEAM 4 /* warps per team (aln_split_team_kernel runs two teams: the forward and the backward pass) */
+#endif
+#ifndef ALN_EMU_TEAMS
+#define ALN_EMU_TEAMS 0
+#endif
+#ifndef ALN_SPLIT_DIGEST
+#define ALN_SPLIT_DIGEST 0
+#endif
+#if ALN_EMU_TEAMS && POA_DEVICE
+#error "ALN_EMU_TEAMS is the host emulation's"
+#endif
+#if ALN_EMU_TEAMS
+struct AlnEmuTeam; /* tests/emu/emu_aln.cpp */
+void aln_emu_barrier(AlnEmuTeam* e, int32_t w);
+void aln_emu_publish(AlnEmuTeam* e, int32_t w, int32_t stripe, int32_t cols_done);
+void aln_emu_wait(AlnEmuTeam* e, int32_t w, int32_t stripe, int32_t cols_needed);
+void aln_emu_hrow_store(AlnEmuTeam* e, int32_t w, const uint32_t* p, int32_t stripe);
+void aln_emu_hrow_load(AlnEmuTeam* e, int32_t w, const uint32_t* p, int32_t stripe, int32_t cols_needed);
+void aln_emu_stripe(AlnEmuTeam* e, int32_t w, int32_t stripe, int32_t c_lo, int32_t c_hi, bool has_other);
+#endif
+#if ALN_SPLIT_DIGEST && !defined(ALN_WAIT_POLLS)
+#define ALN_WAIT_POLLS (1u << 24)
+#endif
 struct TeamCtx {
     int32_t w, n;     /* this warp's place in its team, warps in the team (1: a warp on its own) */
     int32_t bar_id;   /* the team's named barrier (device, n > 1) */
     uint32_t prog_sa; /* shared-memory address of the team's n progress words (device, n > 1) */
+#if ALN_EMU_TEAMS
+    AlnEmuTeam* emu = nullptr; /* the emulated team (null: a warp on its own, nothing to check) */
+#endif
+#if ALN_SPLIT_DIGEST
+    int32_t* timed_out = nullptr; /* set when a team_wait gave up */
+#endif
 };
 POA_FN void team_barrier(const TeamCtx c) {
 #if POA_DEVICE
@@ -261,6 +298,8 @@ POA_FN void team_barrier(const TeamCtx c) {
     } else {
         __syncwarp();
     }
+#elif ALN_EMU_TEAMS
+    if (c.emu && c.n > 1) aln_emu_barrier(c.emu, c.w);
 #else
     (void)c;
 #endif
@@ -270,6 +309,8 @@ POA_FN void team_publish(const TeamCtx c, int32_t stripe, int32_t cols_done) { /
     __threadfence_block();
     const unsigned long long v = ((unsigned long long)(uint32_t)stripe << 32) | (uint32_t)cols_done;
     asm volatile("st.volatile.shared.u64 [%0], %1;" ::"r"(c.prog_sa + 8u * (uint32_t)c.w), "l"(v) : "memory");
+#elif ALN_EMU_TEAMS
+    if (c.emu) aln_emu_publish(c.emu, c.w, stripe, cols_done);
 #else
     (void)c; (void)stripe; (void)cols_done;
 #endif
@@ -279,23 +320,54 @@ POA_FN void team_wait(const TeamCtx c, int32_t stripe, int32_t cols_needed) { /*
     const unsigned long long target = ((unsigned long long)(uint32_t)stripe << 32) | (uint32_t)cols_needed;
     const uint32_t sa = c.prog_sa + 8u * (uint32_t)(stripe % c.n);
     unsigned long long v;
+#if ALN_SPLIT_DIGEST
+    uint32_t polls = 0;
+#endif
     do {
         asm volatile("ld.volatile.shared.u64 %0, [%1];" : "=l"(v) : "r"(sa) : "memory");
+#if ALN_SPLIT_DIGEST
+        if (++polls >= ALN_WAIT_POLLS) {
+            *c.timed_out = 1;
+            break;
+        }
+#endif
     } while (v < target);
     __threadfence_block();
+#elif ALN_EMU_TEAMS
+    if (c.emu) aln_emu_wait(c.emu, c.w, stripe, cols_needed);
 #else
     (void)c; (void)stripe; (void)cols_needed;
 #endif
 }
-/* a word of a hand-over row: written by another warp of the block moments ago, so not through a stale L1 line */
-POA_FN uint32_t hrow_load(const uint32_t* p) {
+/* A word of a hand-over row: written by another warp of the block moments ago, so not through a stale L1 line.
+ * `stripe`: the stripe that must have written it in this pass; `cols_needed`: the columns the consumer's last team_wait
+ * must cover for the word to be complete (emulated teams check both). */
+POA_FN uint32_t hrow_load(const uint32_t* p, const TeamCtx c, int32_t stripe, int32_t cols_needed) {
 #if POA_DEVICE
+    (void)c; (void)stripe; (void)cols_needed;
     uint32_t v;
     asm volatile("ld.volatile.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
     return v;
 #else
+#if ALN_EMU_TEAMS
+    if (c.emu) aln_emu_hrow_load(c.emu, c.w, p, stripe, cols_needed);
+#else
+    (void)c; (void)stripe; (void)cols_needed;
+#endif
     return *p;
 #endif
+}
+/* the columns the stripe above must have run for word k of its hand-over row to be complete: 16 k .. 16 k + 15, or up
+ * to its last column p_hi */
+POA_FN int32_t hrow_word_cols(int32_t k, int32_t p_hi) { return 16 * k + 16 < p_hi + 1 ? 16 * k + 16 : p_hi + 1; }
+/* a word of a hand-over row (or its anchor) written by `stripe`; ONE lane */
+POA_FN void hrow_store(uint32_t* p, uint32_t v, const TeamCtx c, int32_t stripe) {
+#if ALN_EMU_TEAMS
+    if (c.emu) aln_emu_hrow_store(c.emu, c.w, p, stripe);
+#else
+    (void)c; (void)stripe;
+#endif
+    *p = v;
 }
 
 /* The step's shifts on the FMA pipe.  LOP3 / IADD3 / SHF all issue on the ALU pipe (one warp instruction per two cycles
@@ -413,6 +485,9 @@ POA_FN_NOINLINE int64_t myers_pass(const SeqView q, int32_t n, const SeqView t, 
         const int32_t c_hi = band < 0 || R1 + band - 1 > cols - 1 ? cols - 1 : R1 + band - 1;
         const int32_t p_hi = band < 0 || R0 + band - 1 > cols - 1 ? cols - 1 : R0 + band - 1;
         const int32_t a_col = (band < 0 || R1 - band <= 0) ? -1 : R1 - band - 1; /* the anchor column for the stripe below */
+#if ALN_EMU_TEAMS
+        if (team.emu) aln_emu_stripe(team.emu, team.w, sidx, c_lo, c_hi, has_other); /* what the emulated pass ran */
+#endif
         if (c_lo > c_hi) { /* the strip has left the matrix: no row from here on reaches the last column */
             if (out_col) {
                 for (int32_t r = R0 + 1; r <= R1; r += 32) {
@@ -430,9 +505,10 @@ POA_FN_NOINLINE int64_t myers_pass(const SeqView q, int32_t n, const SeqView t, 
         int32_t base_top = lower ? R0 : 0; /* D[R0][c_lo]: the left border's R0 when the strip starts at column 0 */
         if (piped) team_wait(team, sidx - 1, step_first + 32 < p_hi + 1 ? step_first + 32 : p_hi + 1);
         if (lower) {
-            if ((step_first >> 4) <= w_last_in) hword = hrow_load(row_in + (step_first >> 4));
-            if ((step_first >> 4) + 1 <= w_last_in) hword_next = hrow_load(row_in + (step_first >> 4) + 1);
-            if (c_lo > 0) base_top = (int32_t)hrow_load(row_in + (hrow_words - 1));
+            const int32_t k0 = step_first >> 4;
+            if (k0 <= w_last_in) hword = hrow_load(row_in + k0, team, sidx - 1, hrow_word_cols(k0, p_hi));
+            if (k0 + 1 <= w_last_in) hword_next = hrow_load(row_in + k0 + 1, team, sidx - 1, hrow_word_cols(k0 + 1, p_hi));
+            if (c_lo > 0) base_top = (int32_t)hrow_load(row_in + (hrow_words - 1), team, sidx - 1, c_lo); /* at column c_lo - 1 */
         }
         PerLane<uint64_t> Pv, Mv;
         PerLane<int> bot, link, tc_next, hacc;
@@ -504,11 +580,11 @@ POA_FN_NOINLINE int64_t myers_pass(const SeqView q, int32_t n, const SeqView t, 
                 }                                                                                                        \
                 if (more && l == 31) { /* 16 columns to a word; this row's reader is at least 16 columns behind */       \
                     hacc[l] |= out << ((c & 15) * 2);                                                                    \
-                    if (c == a_col) row_out[hrow_words - 1] = (uint32_t)bot[l]; /* the anchor of the stripe below */     \
+                    if (c == a_col) hrow_store(row_out + (hrow_words - 1), (uint32_t)bot[l], team, sidx); /* anchor */   \
                     if ((c & 15) == 15 || c == c_hi) {                                                                   \
                         /* beyond the strip's last column every delta counts + 1 */                                      \
                         if (c == c_hi && (c & 15) != 15) hacc[l] |= (int)(0x55555555u << (((c & 15) + 1) * 2));          \
-                        row_out[c >> 4] = (uint32_t)hacc[l];                                                             \
+                        hrow_store(row_out + (c >> 4), (uint32_t)hacc[l], team, sidx);                                   \
                         hacc[l] = 0;                                                                                     \
                         if (TEAM && team.n > 1 && ((c & 31) == 31 || c == c_hi)) team_publish(team, sidx, c + 1);        \
                     }                                                                                                    \
@@ -526,7 +602,7 @@ POA_FN_NOINLINE int64_t myers_pass(const SeqView q, int32_t n, const SeqView t, 
                 hword_next = 0x55555555u;
                 if (lower && (step0 >> 4) + 1 <= w_last_in) {
                     if (piped) team_wait(team, sidx - 1, p_hi + 1 < step0 + 32 ? p_hi + 1 : step0 + 32);
-                    hword_next = hrow_load(row_in + (step0 >> 4) + 1);
+                    hword_next = hrow_load(row_in + (step0 >> 4) + 1, team, sidx - 1, hrow_word_cols((step0 >> 4) + 1, p_hi));
                 }
             }
             if (!has_other) {
@@ -639,6 +715,53 @@ POA_FN_NOINLINE int64_t aln_split(const AlnSlot& s_ref, EqTab& eq, const uint8_t
     aln_split_rule(s.Lc, s.Rr, n, m, out);
     return cells;
 }
+
+#if ALN_SPLIT_DIGEST || !POA_DEVICE
+/* Test builds: one record per split attempt (b200aln_debug_split_log on the device, the batch emulation in tests/emu),
+ * so that every Hirschberg step -- both middle columns, the split -- can be compared between the two. */
+enum { ALN_PATH_WARP = 0, ALN_PATH_TEAM = 1, ALN_PATH_SIDE = 2 }; /* one warp; a team in a thin level; a team on the side stream */
+enum { ALN_REC_TIMEOUT = 1 };                                      /* flags: a team_wait gave up */
+struct AlnSplitRec {
+    int32_t aln, r0, c0, n, m;
+    int32_t band;    /* what myers_pass got: -1 none */
+    int32_t attempt; /* 0, or 1: redone without a band after a guess that proved too small */
+    int32_t level, path, flags;
+    int32_t r, ls, rs, best;
+    int32_t pad[2];
+    unsigned long long lc_hash, rr_hash; /* aln_col_digest of Lc[0..n] and Rr[0..n] */
+};
+POA_FN unsigned long long aln_mix64(unsigned long long x) { /* splitmix64's finaliser */
+    x ^= x >> 30;
+    x *= 0xbf58476d1ce4e5b9ull;
+    x ^= x >> 27;
+    x *= 0x94d049bb133111ebull;
+    x ^= x >> 31;
+    return x;
+}
+/* Hash of a middle column: the wrapping sum over rows i = 0..n of mix64(i, col[i]), independent of the order lanes visit
+ * the rows in.  Whole warp. */
+POA_FN_NOINLINE unsigned long long aln_col_digest(const int32_t* col, int32_t n) {
+    n = poa_uniform(n);
+    PerLane<unsigned long long> acc;
+    POA_LANES(l) { acc[l] = 0; }
+    for (int32_t base = 0; base <= n; base += 32) {
+        POA_LANES(l) {
+            const int32_t i = base + l;
+            if (i <= n) acc[l] += aln_mix64((((unsigned long long)(uint32_t)i << 32) | (uint32_t)col[i]) + 0x9e3779b97f4a7c15ull);
+        }
+    }
+#if POA_DEVICE
+    unsigned long long t = acc[0];
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) t += __shfl_xor_sync(0xffffffffu, t, d);
+    return t;
+#else
+    unsigned long long t = 0;
+    for (int l = 0; l < 32; ++l) t += acc[l];
+    return t;
+#endif
+}
+#endif
 
 /* ------------------------------------------------------------------------------------------
  * A leaf: store the whole matrix as block records, walk back from the last cell (edlib.cpp:909-1126)

@@ -76,6 +76,11 @@ struct AlnKernelArgs {
     uint8_t* ops;
     AlnResult* res;
     int32_t* counters;
+#if ALN_SPLIT_DIGEST
+    AlnSplitRec* log; /* [log_cap] one record per split attempt (b200aln_debug_split_log) */
+    int32_t* log_count; /* records appended; more than log_cap: the log overflowed */
+    int32_t log_cap;
+#endif
 };
 
 constexpr int WARPS_PER_BLOCK = 2;
@@ -85,6 +90,9 @@ struct AlnWork {
     const AlnRect* list[ALN_CLASSES];
     int32_t n[ALN_CLASSES];
     int32_t total;
+#if ALN_SPLIT_DIGEST
+    int32_t level, path; /* for the split log */
+#endif
 };
 __device__ __forceinline__ AlnRect work_item(const AlnWork& w, int32_t k) {
     if (k < w.n[0]) return w.list[0][k];
@@ -109,6 +117,39 @@ __device__ __forceinline__ int32_t take_work(int32_t* cursor) {
     return __shfl_sync(0xffffffffu, t, 0);
 }
 
+#if ALN_SPLIT_DIGEST
+/* test build: appends the record of one split attempt; whole warp (the hashes), lane 0 holds `sp` */
+__device__ __noinline__ void log_split(const AlnKernelArgs& a, const AlnRect& r, int32_t band, int32_t attempt, int32_t level,
+                                       int32_t path, int32_t flags, const AlnSplit& sp, const int32_t* Lc, const int32_t* Rr) {
+    const unsigned long long lh = aln_col_digest(Lc, r.n), rh = aln_col_digest(Rr, r.n);
+    if ((threadIdx.x & 31u) == 0u) {
+        const int32_t k = atomicAdd(a.log_count, 1);
+        if (k < a.log_cap) {
+            AlnSplitRec x;
+            x.aln = r.aln;
+            x.r0 = r.r0;
+            x.c0 = r.c0;
+            x.n = r.n;
+            x.m = r.m;
+            x.band = band;
+            x.attempt = attempt;
+            x.level = level;
+            x.path = path;
+            x.flags = flags;
+            x.r = sp.r;
+            x.ls = sp.ls;
+            x.rs = sp.rs;
+            x.best = sp.best;
+            x.pad[0] = x.pad[1] = 0;
+            x.lc_hash = lh;
+            x.rr_hash = rh;
+            a.log[k] = x;
+        }
+    }
+    __syncwarp();
+}
+#endif
+
 /* one Hirschberg level: every open sub-problem is split, its children are filed for the next level or as leaves */
 __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, ALN_MIN_BLOCKS) aln_split_kernel(const AlnKernelArgs a, const AlnWork work,
                                                                                         const AlnLists next, int32_t* cursor) {
@@ -124,9 +165,17 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, ALN_MIN_BLOCKS) aln_spli
         const AlnJob job = a.jobs[r.aln];
         AlnSplit sp;
         int64_t cells = aln_split(s, eq, a.seq + job.q_off + r.r0, a.seq + job.t_off + r.c0, r.n, r.m, aln_band_of(r.best), &sp);
+#if ALN_SPLIT_DIGEST
+        log_split(a, r, aln_band_of(r.best), 0, work.level, work.path, 0, sp, s.Lc, s.Rr);
+#endif
         if (r.top & ALN_GUESS) { /* the host's guess was too small? then nothing of that pass can be trusted: no band */
             const int32_t found = __shfl_sync(0xffffffffu, sp.best, 0);
-            if (found > r.best) cells += aln_split(s, eq, a.seq + job.q_off + r.r0, a.seq + job.t_off + r.c0, r.n, r.m, -1, &sp);
+            if (found > r.best) {
+                cells += aln_split(s, eq, a.seq + job.q_off + r.r0, a.seq + job.t_off + r.c0, r.n, r.m, -1, &sp);
+#if ALN_SPLIT_DIGEST
+                log_split(a, r, -1, 1, work.level, work.path, 0, sp, s.Lc, s.Rr);
+#endif
+            }
         }
         if ((threadIdx.x & 31u) == 0u) {
             if (r.top & ALN_TOP) a.res[r.aln].score = sp.best;
@@ -147,9 +196,6 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, ALN_MIN_BLOCKS) aln_spli
  * sub-problem, a team of ALN_TEAM warps on the forward pass and another on the backward pass at the same time, the
  * stripes of a pass pipelined through the team (aln_core.cuh: Teams).  Block workspace: 2 x ALN_TEAM hand-over rows, two
  * code rows, the two middle columns. */
-#ifndef ALN_TEAM
-#define ALN_TEAM 4
-#endif
 #ifndef ALN_TEAM_WAVES
 #define ALN_TEAM_WAVES 4 /* teams while a level's tall sub-problems fit this many waves of team blocks */
 #endif
@@ -179,6 +225,10 @@ __global__ void __launch_bounds__(64 * ALN_TEAM, 1024 / (64 * ALN_TEAM)) aln_spl
     __shared__ uint64_t eq_tab[2 * ALN_TEAM * ALN_EQ_WORDS];
     __shared__ unsigned long long prog[2 * ALN_TEAM];
     __shared__ int32_t s_k, s_redo;
+#if ALN_SPLIT_DIGEST
+    __shared__ int32_t s_timed_out;
+    if (threadIdx.x == 0) s_timed_out = 0;
+#endif
     TeamSlot ts;
     team_slot_bind(ts, a.team_slab + (size_t)blockIdx.x * a.team_slot_bytes, a.max_len, nullptr);
     const int warp = (int)(threadIdx.x >> 5), side = warp / ALN_TEAM; /* side 0: forward pass, side 1: backward pass */
@@ -189,6 +239,9 @@ __global__ void __launch_bounds__(64 * ALN_TEAM, 1024 / (64 * ALN_TEAM)) aln_spl
     team.n = ALN_TEAM;
     team.bar_id = 1 + side;
     team.prog_sa = (uint32_t)__cvta_generic_to_shared(prog + side * ALN_TEAM);
+#if ALN_SPLIT_DIGEST
+    team.timed_out = &s_timed_out;
+#endif
     const int32_t hrow_words = (int32_t)aln_hrow_words(a.max_len);
     for (;;) {
         if (threadIdx.x == 0) s_k = atomicAdd(cursor, 1);
@@ -218,6 +271,10 @@ __global__ void __launch_bounds__(64 * ALN_TEAM, 1024 / (64 * ALN_TEAM)) aln_spl
             if (warp == 0) {
                 aln_split_rule(ts.Lc, ts.Rr, r.n, r.m, &sp);
                 if ((threadIdx.x & 31u) == 0u) s_redo = (attempt == 0 && (r.top & ALN_GUESS) && sp.best > r.best) ? 1 : 0;
+#if ALN_SPLIT_DIGEST
+                log_split(a, r, band, attempt, work.level, work.path, s_timed_out ? ALN_REC_TIMEOUT : 0, sp, ts.Lc, ts.Rr);
+                if ((threadIdx.x & 31u) == 0u) s_timed_out = 0; /* before the next attempt's passes (the barrier below) */
+#endif
             }
             __syncthreads();
             if (!s_redo) break;
@@ -414,6 +471,10 @@ struct b200aln_batch {
     bool aligned = false, synced = false;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     b200aln_batch_info info{};
+#if ALN_SPLIT_DIGEST
+    DevBuf d_log; /* count, then the records of the last align_all (b200aln_debug_split_log) */
+    int32_t log_cap = 0;
+#endif
 };
 
 namespace {
@@ -524,6 +585,9 @@ void b200aln_batch_destroy(b200aln_batch* b) {
     }
     b->d_leaves.release();
     b->d_counters.release();
+#if ALN_SPLIT_DIGEST
+    b->d_log.release();
+#endif
     b->h_seq.release();
     b->h_runs.release();
     b->h_text.release();
@@ -719,6 +783,12 @@ int32_t b200aln_batch_align_all(b200aln_batch* b) {
     }
     ALN_CU(b->d_leaves.need(sizeof(AlnRect) * (size_t)cap_leaves));
     ALN_CU(b->d_counters.need(sizeof(int32_t) * CT_WORDS));
+#if ALN_SPLIT_DIGEST
+    /* a split per open sub-problem (fewer than the leaves) and a redo per alignment at most */
+    b->log_cap = (int32_t)std::min<int64_t>(cap_leaves + n_aln + 64, 0x7FFFFFF);
+    ALN_CU(b->d_log.need(sizeof(AlnSplitRec) * ((size_t)b->log_cap + 1)));
+    ALN_CU(cudaMemsetAsync(b->d_log.p, 0, sizeof(AlnSplitRec), b->stream));
+#endif
 
     cudaStream_t s = b->stream;
     int32_t* ct = static_cast<int32_t*>(b->d_counters.p);
@@ -759,6 +829,11 @@ int32_t b200aln_batch_align_all(b200aln_batch* b) {
     a.ops = static_cast<uint8_t*>(b->d_ops.p);
     a.res = static_cast<AlnResult*>(b->d_res.p);
     a.counters = ct;
+#if ALN_SPLIT_DIGEST
+    a.log_count = static_cast<int32_t*>(b->d_log.p);
+    a.log = static_cast<AlnSplitRec*>(b->d_log.p) + 1;
+    a.log_cap = b->log_cap;
+#endif
     const int32_t max_blocks = b->n_slots / WARPS_PER_BLOCK;
     auto grid_for = [&](int64_t items) {
         return (unsigned)std::max<int64_t>(1, std::min<int64_t>(max_blocks, (items + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK));
@@ -795,9 +870,17 @@ int32_t b200aln_batch_align_all(b200aln_batch* b) {
                 w.total += w.n[slot];
                 ++slot;
             }
+#if ALN_SPLIT_DIGEST
+            w.level = level;
+            w.path = ALN_PATH_WARP;
+#endif
             return w;
         };
-        const auto team = [&](const AlnWork& w, cudaStream_t on) {
+        const auto team = [&](const AlnWork& w_in, cudaStream_t on) {
+            AlnWork w = w_in;
+#if ALN_SPLIT_DIGEST
+            w.path = on == b->side ? ALN_PATH_SIDE : ALN_PATH_TEAM;
+#endif
             if (w.total == 0) return;
             aln_split_team_kernel<<<(unsigned)std::min(w.total, b->n_team_blocks), 64 * ALN_TEAM, 0, on>>>(
                 a, w, next, ct + CT_CURSOR + launch);
@@ -1368,3 +1451,25 @@ int32_t b200aln_aligner_align(b200aln_aligner* h, int64_t n, const uint8_t* q_ba
 }
 
 } // extern "C"
+
+#if ALN_SPLIT_DIGEST
+/* test build only (not part of include/b200aln.h): the split log of the last align_all, one AlnSplitRec per split
+ * attempt in the order the kernels appended them.  *count = records appended; *rec_bytes = sizeof(AlnSplitRec).  Copies
+ * min(count, cap) records to out (nullable).  B200ALN_GENERIC_ERROR when the log overflowed (count > its capacity: the
+ * records beyond it are lost).  Synchronises. */
+extern "C" int32_t b200aln_debug_split_log(b200aln_batch* b, void* out, int64_t cap, int64_t* count, int32_t* rec_bytes) {
+    if (!b || !count) return B200ALN_INVALID_ARGUMENT;
+    if (rec_bytes) *rec_bytes = (int32_t)sizeof(AlnSplitRec);
+    *count = 0;
+    if (!b->aligned || !b->d_log.p) return B200ALN_UNINITIALIZED;
+    ALN_CU(cudaSetDevice(b->device));
+    ALN_CU(cudaStreamSynchronize(b->stream));
+    int32_t n = 0;
+    ALN_CU(cudaMemcpy(&n, b->d_log.p, sizeof(int32_t), cudaMemcpyDeviceToHost));
+    *count = n;
+    const int64_t k = std::min<int64_t>(std::min<int64_t>(n, b->log_cap), cap);
+    if (out && k > 0)
+        ALN_CU(cudaMemcpy(out, static_cast<AlnSplitRec*>(b->d_log.p) + 1, sizeof(AlnSplitRec) * (size_t)k, cudaMemcpyDeviceToHost));
+    return n > b->log_cap ? B200ALN_GENERIC_ERROR : B200ALN_SUCCESS;
+}
+#endif

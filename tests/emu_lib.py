@@ -87,8 +87,51 @@ class EmuAligner:
         n = self.lib.emu_align(C.c_char_p(q), C.c_int32(len(q)), C.c_char_p(t), C.c_int32(len(t)), _p(ops, C.c_uint8),
                                C.byref(score), C.byref(levels), C.byref(leaves), cigar, C.c_int64(cap),
                                C.c_int32(q_first), C.c_int32(t_begin), C.c_int32(window_length), _p(bp, C.c_uint32),
-                               C.byref(bp_count), C.c_int32(guess))
+                               C.byref(bp_count), C.c_int32(guess), C.c_int32(0), None, C.c_int64(0), None)
         self.breaking_points = bp[:2 * bp_count.value].reshape(-1, 2).copy()  # (t, q) pairs, window_length > 0 only
         assert n >= 0, {-1: "inconsistent split", -2: "list overflow", -3: "runs do not spell the operations"}.get(n, n)
         self.cigar = cigar.value
         return ops[:n].copy(), int(score.value), int(levels.value), int(leaves.value)
+
+    def align_log(self, q: bytes, t: bytes, guess: int = -1, aln: int = 0) -> np.ndarray:
+        """The split records (racon_gpu_b200.aligner.SPLIT_REC_DTYPE, path one warp) of aligning one pair as alignment
+        `aln` of a batch, every level and every attempt."""
+        from racon_gpu_b200.aligner import SPLIT_REC_DTYPE
+        assert self.lib.emu_split_rec_bytes() == SPLIT_REC_DTYPE.itemsize
+        cap = 4 * (len(q) * len(t) // (1 << 20) + 4) + 64
+        log = np.zeros(cap, dtype=SPLIT_REC_DTYPE)
+        count = C.c_int64(0)
+        ops = np.zeros(len(q) + len(t) + 8, dtype=np.uint8)
+        score = C.c_int32(-1)
+        n = self.lib.emu_align(C.c_char_p(q), C.c_int32(len(q)), C.c_char_p(t), C.c_int32(len(t)), _p(ops, C.c_uint8),
+                               C.byref(score), None, None, None, C.c_int64(0), C.c_int32(0), C.c_int32(0), C.c_int32(0),
+                               None, None, C.c_int32(guess), C.c_int32(aln), log.ctypes.data_as(C.c_void_p),
+                               C.c_int64(cap), C.byref(count))
+        assert n >= 0 and count.value <= cap, (n, count.value, cap)
+        return log[:count.value].copy()
+
+    #: emu_split's stats, in order
+    SPLIT_STATS = ("stripes", "left_matrix", "anchors", "other", "waits", "failures", "timeouts")
+
+    def split(self, q: bytes, t: bytes, best: int = -1, guess: bool = False, team: bool = False, seed: int = 0):
+        """One Hirschberg step of the sub-problem (q, t) the way a split kernel runs it: one warp, or (team=True) a team
+        block on 2 x ALN_TEAM threads under the protocol checker.  best < 0: no band; guess: best is the host's guess
+        (redone without a band when the optimum is larger).  Returns a list of attempts, each a dict with Lc, Rr (n + 1
+        values), r, ls, rs, best, band; team mode also self.last_stats (SPLIT_STATS) and self.last_failure."""
+        n, m = len(q), len(t)
+        Lc = np.zeros(2 * (n + 1), dtype=np.int32)
+        Rr = np.zeros(2 * (n + 1), dtype=np.int32)
+        sp = np.zeros(8, dtype=np.int32)
+        band = np.zeros(2, dtype=np.int32)
+        stats = np.zeros(7, dtype=np.int64)
+        msg = C.create_string_buffer(512)
+        self.lib.emu_split.restype = C.c_int32
+        k = self.lib.emu_split(C.c_char_p(q), C.c_int32(n), C.c_char_p(t), C.c_int32(m), C.c_int32(best),
+                               C.c_int32(int(guess)), C.c_int32(int(team)), C.c_uint64(seed), _p(Lc, C.c_int32),
+                               _p(Rr, C.c_int32), _p(sp, C.c_int32), _p(band, C.c_int32), _p(stats, C.c_int64), msg,
+                               C.c_int32(512))
+        self.last_stats = dict(zip(self.SPLIT_STATS, stats.tolist()))
+        self.last_failure = msg.value.decode()
+        return [{"Lc": Lc[a * (n + 1):(a + 1) * (n + 1)].copy(), "Rr": Rr[a * (n + 1):(a + 1) * (n + 1)].copy(),
+                 "r": int(sp[4 * a]), "ls": int(sp[4 * a + 1]), "rs": int(sp[4 * a + 2]), "best": int(sp[4 * a + 3]),
+                 "band": int(band[a])} for a in range(k)]

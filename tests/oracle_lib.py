@@ -196,6 +196,15 @@ def oracle_align(oracle: "Oracle", q: bytes, t: bytes):
     return ops[:n].copy(), int(score.value)
 
 
+def oracle_last_column(oracle: "Oracle", q: bytes, t: bytes) -> np.ndarray:
+    """col[i] = D[i][len(t)] of the plain edit-distance matrix of q against t, i = 0..len(q)."""
+    col = np.zeros(len(q) + 1, dtype=np.int32)
+    oracle.lib.aln_oracle_last_column.restype = None
+    oracle.lib.aln_oracle_last_column(C.c_char_p(q), C.c_int32(len(q)), C.c_int(1), C.c_char_p(t), C.c_int32(len(t)),
+                                      C.c_int(1), _p(col, C.c_int32))
+    return col
+
+
 def ops_to_cigar(oracle: "Oracle", ops: np.ndarray) -> bytes:
     ops = np.ascontiguousarray(ops, dtype=np.uint8)
     cap = 16 * ops.shape[0] + 16
