@@ -523,16 +523,42 @@ static poa_graph* subgraph(const poa_graph* g, int32_t begin, int32_t end, int32
     return s;
 }
 
-/* window.cpp:73-116: the graph of one window -- backbone, then every layer aligned (whole graph or subgraph) and added */
+/* Hash of one alignment, the way the engine's test build hashes the one it adds to the graph (poa_core.cuh
+ * aln_digest): the wrapping sum over pairs k (k = 0 leftmost) of mix64(k << 32 | pos << 16 | node), node and pos as
+ * int16 (-1 included), with splitmix64's finaliser as mix64. */
+static uint64_t digest_mix64(uint64_t x) {
+    x ^= x >> 30;
+    x *= 0xbf58476d1ce4e5b9ull;
+    x ^= x >> 27;
+    x *= 0x94d049bb133111ebull;
+    x ^= x >> 31;
+    return x;
+}
+static uint64_t alignment_digest(const poa_pair* aln, int32_t n) {
+    uint64_t t = 0;
+    for (int32_t k = 0; k < n; ++k) {
+        const uint64_t key = (uint64_t)(uint16_t)(int16_t)aln[k].node | ((uint64_t)(uint16_t)(int16_t)aln[k].pos << 16) |
+                             ((uint64_t)(uint32_t)k << 32);
+        t += digest_mix64(key + 0x9e3779b97f4a7c15ull);
+    }
+    return t;
+}
+
+/* window.cpp:73-116: the graph of one window -- backbone, then every layer aligned (whole graph or subgraph) and added.
+ * aln_digest / aln_count (nullable, n_seqs each): per sequence the digest and length of the alignment that was added
+ * (graph ids; 0 and 0 for the backbone). */
 static poa_graph* window_graph(int32_t n_seqs, const char* const* seqs, const int32_t* lens,
                                const int8_t* const* weights, const int32_t* begins, const int32_t* ends,
-                               int32_t m, int32_t x, int32_t gap, int64_t* stats) {
+                               int32_t m, int32_t x, int32_t gap, int64_t* stats, uint64_t* aln_digest,
+                               int32_t* aln_count) {
     int32_t maxlen = 0;
     for (int32_t i = 0; i < n_seqs; ++i)
         if (lens[i] > maxlen) maxlen = lens[i];
     uint32_t* w = (uint32_t*)malloc(sizeof(uint32_t) * (size_t)(maxlen + 1));
 
     poa_graph* g = poa_graph_create();
+    if (aln_digest) aln_digest[0] = 0;
+    if (aln_count) aln_count[0] = 0;
     for (int32_t k = 0; k < lens[0]; ++k) w[k] = weights[0] ? (uint32_t)weights[0][k] : 1u;
     poa_graph_add_alignment(g, NULL, 0, seqs[0], lens[0], w); /* window.cpp:73-76 */
 
@@ -560,6 +586,8 @@ static poa_graph* window_graph(int32_t n_seqs, const char* const* seqs, const in
             poa_graph_destroy(s);
             free(mapping);
         }
+        if (aln_digest) aln_digest[i] = alignment_digest(aln, n_aln);
+        if (aln_count) aln_count[i] = n_aln;
         for (int32_t k = 0; k < lens[i]; ++k) w[k] = weights[i] ? (uint32_t)weights[i][k] : 1u;
         poa_graph_add_alignment(g, aln, n_aln, seqs[i], lens[i], w);
         free(aln);
@@ -583,7 +611,7 @@ int32_t poa_oracle_window_consensus(int32_t n_seqs, const char* const* seqs, con
         if (cov_out) memset(cov_out, 0, sizeof(uint32_t) * (size_t)lens[0]);
         return lens[0];
     }
-    poa_graph* g = window_graph(n_seqs, seqs, lens, weights, begins, ends, m, x, gap, stats);
+    poa_graph* g = window_graph(n_seqs, seqs, lens, weights, begins, ends, m, x, gap, stats, NULL, NULL);
 
     char* cons = NULL;
     uint32_t* cov = NULL;
@@ -667,7 +695,7 @@ int32_t poa_oracle_window_msa(int32_t n_seqs, const char* const* seqs, const int
                               const int8_t* const* weights, const int32_t* begins, const int32_t* ends,
                               int32_t m, int32_t x, int32_t gap, char** rows_out, int32_t* msa_len) {
     if (!ends) begins = NULL;
-    poa_graph* g = window_graph(n_seqs, seqs, lens, weights, begins, ends, m, x, gap, NULL);
+    poa_graph* g = window_graph(n_seqs, seqs, lens, weights, begins, ends, m, x, gap, NULL, NULL, NULL);
     int32_t n = poa_graph_msa(g, rows_out, msa_len);
     poa_graph_destroy(g);
     return n;
@@ -698,6 +726,8 @@ typedef struct {
     int32_t* cons_len;
     uint8_t* polished;
     int64_t* stats;
+    uint64_t* aln_digest; /* set: the job digests alignments (poa_oracle_alignment_digests) instead of polishing */
+    int32_t* aln_count;
     int64_t cursor;
     pthread_mutex_t mu;
 } batch_job;
@@ -733,6 +763,11 @@ static void* batch_worker(void* arg) {
             bg[k] = job->begins[s];
             en[k] = job->ends[s];
         }
+        if (job->aln_digest) {
+            poa_graph_destroy(window_graph(n, seqs, lens, wts, bg, en, job->m, job->x, job->gap, NULL,
+                                           job->aln_digest + s0, job->aln_count + s0));
+            continue;
+        }
         int32_t pol = 0;
         int32_t len = poa_oracle_window_consensus(
             n, seqs, lens, wts, bg, en, job->tgs, job->trim, job->m, job->x, job->gap,
@@ -751,6 +786,42 @@ static void* batch_worker(void* arg) {
     free(bg);
     free(en);
     return NULL;
+}
+
+static void run_batch_job(batch_job* job, int32_t n_threads) {
+    pthread_mutex_init(&job->mu, NULL);
+    if (n_threads <= 1) {
+        batch_worker(job);
+    } else {
+        pthread_t* th = (pthread_t*)malloc(sizeof(pthread_t) * (size_t)n_threads);
+        for (int32_t t = 0; t < n_threads; ++t) pthread_create(&th[t], NULL, batch_worker, job);
+        for (int32_t t = 0; t < n_threads; ++t) pthread_join(th[t], NULL);
+        free(th);
+    }
+    pthread_mutex_destroy(&job->mu);
+}
+
+void poa_oracle_alignment_digests(int64_t n_windows, const int64_t* win_seq_off, const int64_t* seq_off,
+                                  const uint8_t* bases, const int8_t* weights, const uint8_t* has_weights,
+                                  const int32_t* begins, const int32_t* ends, const int32_t* order, int32_t m,
+                                  int32_t x, int32_t gap, int32_t n_threads, uint64_t* aln_digest, int32_t* aln_count) {
+    batch_job job;
+    memset(&job, 0, sizeof(job));
+    job.n_windows = n_windows;
+    job.win_seq_off = win_seq_off;
+    job.seq_off = seq_off;
+    job.bases = bases;
+    job.weights = weights;
+    job.has_weights = has_weights;
+    job.begins = begins;
+    job.ends = ends;
+    job.order = order;
+    job.m = m;
+    job.x = x;
+    job.gap = gap;
+    job.aln_digest = aln_digest;
+    job.aln_count = aln_count;
+    run_batch_job(&job, n_threads);
 }
 
 void poa_oracle_polish_windows(int64_t n_windows, const int64_t* win_seq_off, const int64_t* seq_off,
@@ -782,16 +853,7 @@ void poa_oracle_polish_windows(int64_t n_windows, const int64_t* win_seq_off, co
     job.cons_len = cons_len;
     job.polished = polished;
     job.stats = stats;
-    pthread_mutex_init(&job.mu, NULL);
-    if (n_threads <= 1) {
-        batch_worker(&job);
-    } else {
-        pthread_t* th = (pthread_t*)malloc(sizeof(pthread_t) * (size_t)n_threads);
-        for (int32_t t = 0; t < n_threads; ++t) pthread_create(&th[t], NULL, batch_worker, &job);
-        for (int32_t t = 0; t < n_threads; ++t) pthread_join(th[t], NULL);
-        free(th);
-    }
-    pthread_mutex_destroy(&job.mu);
+    run_batch_job(&job, n_threads);
 }
 
 /* ------------------------------------------------------------------------------------------------

@@ -89,6 +89,15 @@ void poa_oracle_polish_windows(int64_t n_windows, const int64_t* win_seq_off, co
                                uint16_t* cov_out, int32_t stride, int32_t* cons_len,
                                uint8_t* polished, int64_t* stats);
 
+/* The alignments spoa adds to each window's graph, same flat layout and processing order as
+ * poa_oracle_polish_windows: per sequence (ADD-order index of its window's first sequence + processing position) the
+ * wrapping sum over pairs k (k = 0 leftmost) of mix64(k << 32 | (uint16)pos << 16 | (uint16)node) with graph node ids
+ * (a subgraph alignment mapped back, graph.cpp:675-683) and the number of pairs; 0 and 0 for the backbone. */
+void poa_oracle_alignment_digests(int64_t n_windows, const int64_t* win_seq_off, const int64_t* seq_off,
+                                  const uint8_t* bases, const int8_t* weights, const uint8_t* has_weights,
+                                  const int32_t* begins, const int32_t* ends, const int32_t* order, int32_t m,
+                                  int32_t x, int32_t gap, int32_t n_threads, uint64_t* aln_digest, int32_t* aln_count);
+
 /* spoa::Graph::generate_multiple_sequence_alignment(dst, false)  (graph.cpp:373-427): one row per sequence in the
  * order they were added, '-' where the sequence has no base in a column.  *rows_out is one malloc'ed block of
  * n_rows x *msa_len bytes (free with poa_oracle_free); returns n_rows. */

@@ -72,6 +72,10 @@ struct KernelArgs {
     unsigned long long* fill_digest; /* [staged sequences] see b200poa_debug_fill_digest */
     int32_t* fill_count;
 #endif
+#if POA_ALN_DIGEST
+    unsigned long long* aln_digest;  /* [staged sequences] see b200poa_debug_aln_digest */
+    int32_t* aln_count;
+#endif
 };
 
 #ifndef POA_MIN_BLOCKS_PER_SM
@@ -128,6 +132,10 @@ __global__ void __launch_bounds__(32, POA_MIN_BLOCKS_PER_SM) poa_window_kernel(c
 #if POA_FILL_DIGEST
         wv.fill_digest = a.fill_digest + s0;
         wv.fill_count = a.fill_count + s0;
+#endif
+#if POA_ALN_DIGEST
+        wv.aln_digest = a.aln_digest + s0;
+        wv.aln_count = a.aln_count + s0;
 #endif
         WindowOut out;
         out.cons = a.out_cons;
@@ -262,6 +270,10 @@ struct b200poa_batch {
     unsigned long long* d_fill_digest = nullptr; /* [max_seqs] per staged sequence, see b200poa_debug_fill_digest */
     int32_t* d_fill_count = nullptr;
 #endif
+#if POA_ALN_DIGEST
+    unsigned long long* d_aln_digest = nullptr; /* [max_seqs] see b200poa_debug_aln_digest */
+    int32_t* d_aln_count = nullptr;
+#endif
     size_t msa_cap = 0;
     size_t msa_bound = 0;                  /* worst-case MSA bytes of the windows staged so far */
     bool msa_fetched = false;
@@ -377,6 +389,10 @@ static void free_batch(b200poa_batch* b) {
 #if POA_FILL_DIGEST
     cudaFree(b->d_fill_digest);
     cudaFree(b->d_fill_count);
+#endif
+#if POA_ALN_DIGEST
+    cudaFree(b->d_aln_digest);
+    cudaFree(b->d_aln_count);
 #endif
     delete b;
 }
@@ -578,6 +594,10 @@ static int32_t alloc_batch_memory(b200poa_batch* b) {
 #if POA_FILL_DIGEST
     CU_TRY(cudaMalloc(&b->d_fill_digest, (MS + 1) * sizeof(unsigned long long)));
     CU_TRY(cudaMalloc(&b->d_fill_count, (MS + 1) * sizeof(int32_t)));
+#endif
+#if POA_ALN_DIGEST
+    CU_TRY(cudaMalloc(&b->d_aln_digest, (MS + 1) * sizeof(unsigned long long)));
+    CU_TRY(cudaMalloc(&b->d_aln_count, (MS + 1) * sizeof(int32_t)));
 #endif
     return B200POA_SUCCESS;
 }
@@ -967,6 +987,12 @@ int32_t b200poa_batch_launch(b200poa_batch* b) {
     a.fill_digest = b->d_fill_digest;
     a.fill_count = b->d_fill_count;
 #endif
+#if POA_ALN_DIGEST
+    CU_TRY(cudaMemsetAsync(b->d_aln_digest, 0, (size_t)b->seq_count * sizeof(unsigned long long), b->stream));
+    CU_TRY(cudaMemsetAsync(b->d_aln_count, 0, (size_t)b->seq_count * sizeof(int32_t), b->stream));
+    a.aln_digest = b->d_aln_digest;
+    a.aln_count = b->d_aln_count;
+#endif
     /* persistent grid: one warp per resident slot.  (Shrinking the grid so that every round of it is full --
      * 10000 windows as 3 x 3334 instead of 2.8 x 3552 -- was measured neutral: throughput follows the number of
      * resident warps.  B200POA_GRID_BALANCE=1 keeps the experiment available.) */
@@ -1150,6 +1176,18 @@ extern "C" int32_t b200poa_debug_fill_digest(b200poa_batch* b, uint64_t* digest,
     CU_TRY(cudaMemcpy(count, b->d_fill_count, (size_t)b->seq_count * sizeof(int32_t), cudaMemcpyDeviceToHost));
     if (ring_rows) *ring_rows = b->ring_rows;
     if (ring_stride) *ring_stride = b->ring_stride;
+    return B200POA_SUCCESS;
+}
+#endif
+#if POA_ALN_DIGEST
+/* test build only: after the last launch, per staged sequence (same order as b200poa_debug_fill_digest) aln_digest() of
+ * the alignment added to the graph and its entry count; 0 and 0 for backbones and for reads never added.  Synchronises. */
+extern "C" int32_t b200poa_debug_aln_digest(b200poa_batch* b, uint64_t* digest, int32_t* count, int64_t n) {
+    if (!b || !digest || !count || n < b->seq_count) return B200POA_INVALID_ARGUMENT;
+    DeviceGuard g(b->device);
+    CU_TRY(cudaStreamSynchronize(b->stream));
+    CU_TRY(cudaMemcpy(digest, b->d_aln_digest, (size_t)b->seq_count * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+    CU_TRY(cudaMemcpy(count, b->d_aln_count, (size_t)b->seq_count * sizeof(int32_t), cudaMemcpyDeviceToHost));
     return B200POA_SUCCESS;
 }
 #endif

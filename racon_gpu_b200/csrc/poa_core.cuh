@@ -45,6 +45,25 @@
 #ifndef POA_FILL_DIGEST
 #define POA_FILL_DIGEST 0
 #endif
+/* Test build (-DPOA_ALN_DIGEST=1, the same library and tests/emu): the alignment every read adds to the graph is hashed
+ * (aln_digest) so that the traceback can be compared read for read with its scalar twin and with spoa.  A define of its
+ * own: a caller that fills only the fill-digest fields of WindowView stays correct. */
+#ifndef POA_ALN_DIGEST
+#define POA_ALN_DIGEST 0
+#endif
+
+/* Hooks of the emulation (tests/emu): POA_TB_REACH(field) counts a path of the traceback, POA_TB_REACH_IF(cond, field)
+ * counts it when cond holds, and POA_TB_TWIN(fill, ...) checks every traceback against a scalar twin walk.  Elsewhere
+ * they expand to nothing (cond is not evaluated): no kernel, the digest build included, contains them. */
+#ifndef POA_TB_REACH
+#define POA_TB_REACH(field) ((void)0)
+#endif
+#ifndef POA_TB_REACH_IF
+#define POA_TB_REACH_IF(cond, field) ((void)0)
+#endif
+#ifndef POA_TB_TWIN
+#define POA_TB_TWIN(fill, ...) ((void)0)
+#endif
 
 namespace b200poa {
 
@@ -248,6 +267,11 @@ struct WindowView {
 #if POA_FILL_DIGEST
     unsigned long long* fill_digest; /* [n_seqs] test build only: sum of fill_digest() over every fill of the sequence */
     int32_t* fill_count;             /* [n_seqs] fills of the sequence (adaptive retries included) */
+#endif
+#if POA_ALN_DIGEST
+    unsigned long long* aln_digest;  /* [n_seqs] test build only: aln_digest() of the alignment added to the graph
+                                        (last adaptive try) */
+    int32_t* aln_count;              /* [n_seqs] its entries */
 #endif
 };
 
@@ -1186,6 +1210,7 @@ POA_FN_NOINLINE int32_t traceback_i32(const Slot& s_ref, const Params p, WinStat
     const int32_t cap = p.max_nodes + p.max_len + 2, stride = p.stride, bw = g.bw;
     const int32_t mg = p.match - p.gap, xg = p.mismatch - p.gap;
     int32_t w = cap, lost = 0;
+    POA_TB_REACH(i32_reads);
     POA_LANE0 {
         int32_t i = end_row, j = g.len;
         while (!(i == 0 && j == 0) && !lost) {
@@ -1397,6 +1422,23 @@ POA_FN uint32_t tile_u16(tile_addr a, int32_t i) { return reinterpret_cast<const
 POA_FN uint32_t tile_u8(tile_addr a, int32_t i) { return a[i]; }
 #endif
 
+/* Reach report of the emulation (POA_TB_REACH_IF): does the step at (i, j) read a tile chunk the load filled with NEG,
+ * i.e. a cell of row i at j - 1 or of a predecessor at j or j - 1 outside that row's band?  (Band starts and the tile's
+ * chunks are 8-aligned: a chunk lies wholly inside its row's band or wholly outside.) */
+POA_FN bool tb_out_of_band(const ReadGeom& g, int32_t row, int32_t col) {
+    const int32_t o = col - band_start(g, row, g.n_rows);
+    return g.banded && col >= 0 && (o < 0 || o >= g.bw);
+}
+POA_FN bool tb_step_reads_neg_chunk(const ReadGeom& g, const uint32_t* row_poff, const uint32_t* row_pred, int32_t i,
+                                    int32_t j, int32_t np) {
+    bool neg = j > 0 && tb_out_of_band(g, i, j - 1);
+    for (int32_t k = 0; k < np; ++k) {
+        const int32_t pi = (int32_t)(row_pred[row_poff[i] + k] & 0xFFFFu);
+        neg = neg || tb_out_of_band(g, pi, j) || (j > 0 && tb_out_of_band(g, pi, j - 1));
+    }
+    return neg;
+}
+
 POA_FN void tb_bind(TbScratch& t, uint8_t* base) {
     t.cells = reinterpret_cast<int16_t*>(base);
     base += TB_ROWS * TB_COLS * 2;
@@ -1474,6 +1516,8 @@ POA_FN_NOINLINE int32_t traceback(const Slot& s, const Params p, WinState& st, c
             return cap;
         }
         if (i == 0) { /* first row: S[0][*] == 0, only horizontal moves are left */
+            POA_TB_REACH_IF(j >= 32, row0_tail32);
+            POA_TB_REACH_IF(j >= 64, row0_tail64);
             POA_TB_FLUSH();
             for (int32_t b = 0; b < j; b += 32) {
                 POA_LANES(l) {
@@ -1497,14 +1541,17 @@ POA_FN_NOINLINE int32_t traceback(const Slot& s, const Params p, WinState& st, c
         bool reloaded = false;
         if (i > r_hi || i < r_lo || j > c_hi || (j > 0 && j - 1 < c_lo)) {
             POA_SUB_LAP(11);
+            POA_TB_REACH(tile_loads);
             r_hi = i;
             r_lo = i - (TB_ROWS - 1) < 0 ? 0 : i - (TB_ROWS - 1);
             c_hi = j;
             c_lo = ((j + 1 - TB_COLS) < 0 ? 0 : (j + 1 - TB_COLS + 7)) & ~7; /* 8-aligned, covers j */
             if (gg.banded && pu.adaptive) { /* adaptive band: is the path (sampled once per tile) about to leave the band? */
                 const int32_t bs_i = band_start(gg, i, gg.n_rows);
-                if ((bs_i > 0 && j - bs_i < TB_EDGE_MARGIN) || (bs_i + bw < gg.colsP && bs_i + bw - 1 - j < TB_EDGE_MARGIN))
+                if ((bs_i > 0 && j - bs_i < TB_EDGE_MARGIN) || (bs_i + bw < gg.colsP && bs_i + bw - 1 - j < TB_EDGE_MARGIN)) {
                     st.band_hit = 1;
+                    POA_TB_REACH(band_hits);
+                }
             }
             POA_SYNC();
             /* ONE round of independent loads.  The band start of a row is recomputed (same formula as the
@@ -1645,6 +1692,8 @@ POA_FN_NOINLINE int32_t traceback(const Slot& s, const Params p, WinState& st, c
         uint32_t node_i = info >> 16;
         if (tp != 0xFF) {
             /* the common row (one in-edge, source in the tile): warp-uniform scalar code on four tile reads */
+            POA_TB_REACH(common_steps);
+            POA_TB_REACH_IF(tb_step_reads_neg_chunk(gg, row_poff, row_pred, i, j, 1), neg_chunk_steps);
             const int32_t x = j - c_lo; /* >= 1 unless j == 0 */
             const int32_t cb = tp * TB_COLS + x;
             const int32_t vv = tile_s16(A_cells, cb);
@@ -1710,12 +1759,20 @@ POA_FN_NOINLINE int32_t traceback(const Slot& s, const Params p, WinState& st, c
                 found = 1;
             }
         }
+        if (in_tile) {
+            POA_TB_REACH(tile_steps);
+            POA_TB_REACH_IF(tb_step_reads_neg_chunk(gg, row_poff, row_pred, i, j, np), neg_chunk_steps);
+        }
         if (!in_tile) {
             if (!reloaded) { /* a predecessor fell off the tile: re-anchor the tile at (i, j) and retry */
+                POA_TB_REACH(reanchors);
                 r_hi = -1;
                 continue;
             }
             /* even a tile anchored here does not hold the step: read global memory directly */
+            POA_TB_REACH_IF(np > 32, global_npred);
+            POA_TB_REACH_IF(np <= 32 && po - pred_base + np > pred_n, global_pred_cap);
+            POA_TB_REACH_IF(np <= 32 && po - pred_base + np <= pred_n, global_far);
             const int32_t gpo = (int32_t)row_poff[i];
             for (int pass = 0; pass < 2 && !found; ++pass) { /* pass 0: diagonal, pass 1: vertical */
                 for (int32_t b = 0; b < np && !found; b += 32) {
@@ -2705,7 +2762,7 @@ POA_HD bool score_range_ok(const Params& p, int32_t n_columns, int32_t len) {
     return lo > NEG + 512 && hi < 32000;
 }
 
-#if POA_FILL_DIGEST
+#if POA_FILL_DIGEST || POA_ALN_DIGEST
 POA_FN unsigned long long digest_mix64(unsigned long long x) { /* splitmix64's finaliser */
     x ^= x >> 30;
     x *= 0xbf58476d1ce4e5b9ull;
@@ -2714,6 +2771,20 @@ POA_FN unsigned long long digest_mix64(unsigned long long x) { /* splitmix64's f
     x ^= x >> 31;
     return x;
 }
+POA_FN unsigned long long digest_warp_sum(const PerLane<unsigned long long>& acc) {
+#if POA_DEVICE
+    unsigned long long t = acc[0];
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) t += __shfl_xor_sync(0xffffffffu, t, d);
+    return t;
+#else
+    unsigned long long t = 0;
+    for (int l = 0; l < 32; ++l) t += acc[l];
+    return t;
+#endif
+}
+#endif
+#if POA_FILL_DIGEST
 /* Hash of the score rows the fill of one read just wrote: the wrapping sum, over the real cells (rows 1..n_rows, columns
  * [band start, band start + bw) within [0, len]), of mix64(row, column, value).  A sum does not depend on the order in
  * which lanes visit cells.  Cells past the read are not specified by the fill's contract and are not hashed. */
@@ -2735,16 +2806,27 @@ POA_FN_NOINLINE unsigned long long fill_digest(const Slot& s_ref, const Params p
             }
         }
     }
-#if POA_DEVICE
-    unsigned long long t = acc[0];
-#pragma unroll
-    for (int d = 16; d > 0; d >>= 1) t += __shfl_xor_sync(0xffffffffu, t, d);
-    return t;
-#else
-    unsigned long long t = 0;
-    for (int l = 0; l < 32; ++l) t += acc[l];
-    return t;
+    return digest_warp_sum(acc);
+}
 #endif
+#if POA_ALN_DIGEST
+/* Hash of the alignment the traceback left in tb_node/tb_pos[tb, cap): the wrapping sum over entries k (k = 0 is the
+ * leftmost) of mix64(k << 32 | (uint16)pos << 16 | (uint16)node), -1 included.  The oracle hashes spoa's alignments the
+ * same way (poa_oracle_alignment_digests). */
+POA_FN_NOINLINE unsigned long long aln_digest(const Slot& s_ref, const Params p, int32_t tb) {
+    const Slot s = s_ref;
+    const int32_t cap = p.max_nodes + p.max_len + 2;
+    PerLane<unsigned long long> acc;
+    POA_LANES(l) {
+        acc[l] = 0;
+        for (int32_t e = tb + l; e < cap; e += 32) {
+            const unsigned long long key = (unsigned long long)(uint16_t)s.tb_node[e] |
+                                           ((unsigned long long)(uint16_t)s.tb_pos[e] << 16) |
+                                           ((unsigned long long)(uint32_t)(e - tb) << 32);
+            acc[l] += digest_mix64(key + 0x9e3779b97f4a7c15ull);
+        }
+    }
+    return digest_warp_sum(acc);
 }
 #endif
 
@@ -2875,6 +2957,7 @@ POA_FN int32_t process_window(const Slot& s, const Params& p, const WindowView& 
                 winstate_uniform(st);
                 POA_FENCE();
                 tm.lap(PH_TRACEBACK);
+                POA_TB_TWIN(fill, s, p, st, g, r, read, end_row, tb, partial ? s.sub_at : s.node_at, cells32, partial);
             }
             if (p.adaptive && g.banded && (st.band_hit || st.status == ST_TRACEBACK_LOST)) {
                 st.status = ST_SUCCESS;
@@ -2884,6 +2967,16 @@ POA_FN int32_t process_window(const Slot& s, const Params& p, const WindowView& 
             break;
         }
         if (st.status != ST_SUCCESS) break;
+#if POA_ALN_DIGEST
+        {
+            const unsigned long long d = aln_digest(s, p, tb);
+            POA_LANE0 {
+                wv.aln_digest[r] = d;
+                wv.aln_count[r] = p.max_nodes + p.max_len + 2 - tb;
+            }
+            POA_SYNC();
+        }
+#endif
 #if POA_DEVICE && POA_PREFETCH_GRAPH == 3
         prefetch_graph(s, poa_uniform(st.n_nodes), poa_uniform(st.n_edges));
 #endif

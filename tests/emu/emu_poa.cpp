@@ -8,6 +8,7 @@
  * per-root topological sort, consensus) and the band definition are checked without a GPU.
  * Never linked into the product library.
  */
+#include <algorithm>
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
@@ -16,11 +17,102 @@
 #include <atomic>
 #include <vector>
 
+/* Traceback reach report: per window, how often the traceback took each of its paths (tests/emu_lib.py names the
+ * fields, tests/tb_cases.py reads them).  traceback() and traceback_i32() count through POA_TB_REACH; the twin check
+ * after every traceback (ScalarFill::traceback_twin) counts the rest. */
+enum TbReach {
+    TB_tracebacks = 0, /* tracebacks run (every adaptive try)                                              */
+    TB_tile_loads,     /* tiles loaded                                                                     */
+    TB_reanchors,      /* tiles re-anchored at the current cell because a step's data was not in the tile   */
+    TB_global_npred,   /* steps read from global memory: more than 32 in-edges                              */
+    TB_global_pred_cap,/* ... <= 32 in-edges, but CSR entries past TB_PRED_CAP                              */
+    TB_global_far,     /* ... a predecessor more than TB_ROWS - 1 rows back after the re-anchor             */
+    TB_common_steps,   /* steps of a row with one in-edge whose source is in the tile                      */
+    TB_tile_steps,     /* other steps resolved in the tile                                                 */
+    TB_neg_chunk_steps,/* tile steps that read a NEG-filled chunk (out of the row's band)                  */
+    TB_band_hits,      /* adaptive band: tiles anchored within TB_EDGE_MARGIN of a band edge               */
+    TB_row0_tail32,    /* tracebacks with a row-0 tail of 32 or more horizontal moves                      */
+    TB_row0_tail64,    /* ... of 64 or more                                                                */
+    TB_vrun32,         /* tracebacks with a run of 32 or more vertical moves                               */
+    TB_count_mod0,     /* tracebacks whose entry count is 0 mod 32                                         */
+    TB_count_mod1,     /* ... 1 mod 32                                                                     */
+    TB_count_mod31,    /* ... 31 mod 32                                                                    */
+    TB_i32_reads,      /* tracebacks on 32-bit cells (traceback_i32)                                       */
+    TB_partial_reads,  /* tracebacks against a subgraph (partial-span layer)                               */
+    TB_twin_mismatches,/* tracebacks whose alignment differs from the scalar twin's                        */
+    TB_FIELDS
+};
+thread_local int32_t* tb_reach_now = nullptr; /* the window the calling thread works on, or nullptr */
+#define POA_TB_REACH(field) (tb_reach_now ? (void)(tb_reach_now[TB_##field] += 1) : (void)0)
+#define POA_TB_REACH_IF(cond, field) ((cond) ? POA_TB_REACH(field) : (void)0)
+#define POA_TB_TWIN(fill, ...) (fill).traceback_twin(__VA_ARGS__)
+#define POA_ALN_DIGEST 1 /* WindowView::aln_digest / aln_count: set for every window below */
+
 #include "../../racon_gpu_b200/csrc/poa_core.cuh"
 
 using namespace b200poa;
 
 namespace {
+
+/* Scalar twin of the traceback (traceback() and traceback_i32()): spoa's priority -- diagonal over the in-edges in
+ * order, then vertical over the in-edges in order, then horizontal -- walked one cell at a time on the same slot
+ * matrix, re-reading every cell; no tile, no lanes, no output buffer.  Entries leftmost first; false if the band holds
+ * no consistent path. */
+struct ScalarTraceback {
+    static bool walk(const Slot& s, const Params& p, const ReadGeom& g, const uint8_t* read, int32_t end_row,
+                     const uint16_t* row_node, bool cells32, std::vector<int16_t>& node, std::vector<int16_t>& pos) {
+        const int32_t* S32 = reinterpret_cast<const int32_t*>(s.S);
+        const auto cell = [&](int32_t row, int32_t bs, int32_t col) -> int32_t {
+            return cells32 ? cell32(S32, p.stride, g.bw, row, bs, col) : score_at_bs(s, p, g, row, bs, col);
+        };
+        const int32_t mg = p.match - p.gap, xg = p.mismatch - p.gap;
+        node.clear();
+        pos.clear();
+        int32_t i = end_row, j = g.len;
+        while (!(i == 0 && j == 0)) {
+            int32_t ni = i, nj = j;
+            if (i == 0) {
+                nj = j - 1;
+            } else {
+                const uint32_t rec = s.row_rec[i];
+                const int32_t np = rec_npred(rec), bs = rec_bs(rec), po = (int32_t)s.row_poff[i];
+                const int32_t cur = cell(i, bs, j);
+                const int32_t prof = (j > 0 && rec_code(rec) == (int32_t)read[j - 1]) ? mg : xg;
+                bool found = false;
+                for (int32_t k = 0; k < np && !found && j > 0; ++k) {
+                    const uint32_t pe = s.row_pred[po + k];
+                    if (cell((int32_t)(pe & 0xFFFFu), (int32_t)(pe >> 16), j - 1) + prof == cur) {
+                        ni = (int32_t)(pe & 0xFFFFu);
+                        nj = j - 1;
+                        found = true;
+                    }
+                }
+                for (int32_t k = 0; k < np && !found; ++k) {
+                    const uint32_t pe = s.row_pred[po + k];
+                    if (cell((int32_t)(pe & 0xFFFFu), (int32_t)(pe >> 16), j) + p.gap == cur) {
+                        ni = (int32_t)(pe & 0xFFFFu);
+                        found = true;
+                    }
+                }
+                if (!found) {
+                    if (j > 0 && cell(i, bs, j - 1) == cur) nj = j - 1;
+                    else return false;
+                }
+            }
+            node.push_back((int16_t)(i == ni ? -1 : (int32_t)row_node[i - 1]));
+            pos.push_back((int16_t)(j == nj ? -1 : j - 1));
+            i = ni;
+            j = nj;
+        }
+        std::reverse(node.begin(), node.end());
+        std::reverse(pos.begin(), pos.end());
+        return true;
+    }
+};
+
+/* the first traceback of a window that differs from its twin: read (processing position), try, entry index, the twin's
+ * entry (node, pos), the engine's entry, the twin's and the engine's entry counts (-1: lost; entry -2: none) */
+constexpr int TB_MISMATCH_INTS = 9;
 
 /* Reach report: per window, which paths of the CUDA fill its reads would take (tests/fill_cases.py names the fields). */
 enum Reach {
@@ -44,6 +136,50 @@ struct ScalarFill {
     int64_t cells = 0;
     int32_t* reach = nullptr; /* this window's report, or nullptr */
     const uint8_t* last_read = nullptr;
+    int32_t* tb_reach = nullptr;    /* this window's traceback report (TB_FIELDS), or nullptr */
+    int32_t* tb_mismatch = nullptr; /* this window's first twin mismatch (TB_MISMATCH_INTS), or nullptr */
+    const uint8_t* tb_last_read = nullptr;
+    int32_t tb_try = 0;
+    std::vector<int16_t> twin_node, twin_pos;
+
+    /* POA_TB_TWIN: after every traceback of process_window(), walk the twin on the same matrix and compare */
+    void traceback_twin(const Slot& s, const Params& p, const WinState& st, const ReadGeom& g, int32_t r,
+                        const uint8_t* read, int32_t end_row, int32_t tb, const uint16_t* row_node, bool cells32,
+                        bool partial) {
+        tb_try = read == tb_last_read ? tb_try + 1 : 0;
+        tb_last_read = read;
+        const int32_t cap = p.max_nodes + p.max_len + 2;
+        const bool lost = st.status == ST_TRACEBACK_LOST;
+        const int32_t n = lost ? -1 : cap - tb;
+        const bool twin_ok = ScalarTraceback::walk(s, p, g, read, end_row, row_node, cells32, twin_node, twin_pos);
+        const int32_t tn = twin_ok ? (int32_t)twin_node.size() : -1;
+        int32_t k = 0; /* first differing entry */
+        while (k < n && k < tn && twin_node[(size_t)k] == s.tb_node[tb + k] && twin_pos[(size_t)k] == s.tb_pos[tb + k]) ++k;
+        const bool same = tn == n && k == std::max(n, 0);
+        if (tb_reach) {
+            int32_t* t = tb_reach;
+            t[TB_tracebacks] += 1;
+            if (!same) t[TB_twin_mismatches] += 1;
+            if (partial) t[TB_partial_reads] += 1;
+            if (n >= 0) {
+                t[TB_count_mod0] += n % 32 == 0;
+                t[TB_count_mod1] += n % 32 == 1;
+                t[TB_count_mod31] += n % 32 == 31;
+                int32_t run = 0, longest = 0;
+                for (int32_t e = tb; e < cap; ++e) {
+                    run = (s.tb_pos[e] == -1 && s.tb_node[e] != -1) ? run + 1 : 0;
+                    longest = std::max(longest, run);
+                }
+                t[TB_vrun32] += longest >= 32;
+            }
+        }
+        if (!same && tb_mismatch && tb_mismatch[0] < 0) {
+            const int32_t m[TB_MISMATCH_INTS] = {r, tb_try, k, k < tn ? twin_node[(size_t)k] : -2, k < tn ? twin_pos[(size_t)k] : -2,
+                                                 k < n ? s.tb_node[tb + k] : -2, k < n ? s.tb_pos[tb + k] : -2, tn, n};
+            std::copy(m, m + TB_MISMATCH_INTS, tb_mismatch);
+        }
+    }
+
     int32_t operator()(const Slot& s, const Params& p, WinState& st, const ReadGeom& g,
                        const uint8_t* read) {
         const int32_t N = g.n_rows;
@@ -122,8 +258,9 @@ extern "C" {
 
 /* Flat batch in ADD order + order[] (processing permutation), like poa_oracle_polish_windows.
  * Outputs the UNTRIMMED consensus, coverage and the per-window status.  rank_out (nullable):
- * n_windows x max_nodes final rank_to_node order, n_nodes_out (nullable) node counts. */
-void emu_polish_windows(int64_t n_windows, const int64_t* win_seq_off, const int64_t* seq_off,
+ * n_windows x max_nodes final rank_to_node order, n_nodes_out (nullable) node counts.  emu_polish_windows (below) is
+ * the same without the traceback's outputs. */
+void emu_polish_windows_tb(int64_t n_windows, const int64_t* win_seq_off, const int64_t* seq_off,
                         const uint8_t* bases, const int8_t* weights, const uint8_t* has_weights,
                         const int32_t* begins, const int32_t* ends, const int32_t* order, int32_t m, int32_t x, int32_t gap,
                         int32_t max_nodes, int32_t max_edges, int32_t max_len, int32_t band_width,
@@ -135,7 +272,12 @@ void emu_polish_windows(int64_t n_windows, const int64_t* win_seq_off, const int
                         /* ring_rows: the score-row ring of the GPU launch to compare with (the row program's far-predecessor
                          * flags depend on it).  Per sequence (window by window, processing order; nullable): the sum of
                          * fill_digest() over its fills and their number.  Per window (nullable): R_FIELDS reach counters. */
-                        int32_t ring_rows, unsigned long long* digest_out, int32_t* fill_count_out, int32_t* reach_out) {
+                        int32_t ring_rows, unsigned long long* digest_out, int32_t* fill_count_out, int32_t* reach_out,
+                        /* Per sequence (nullable): aln_digest() of the alignment added to the graph and its entry
+                         * count.  Per window (nullable): TB_FIELDS traceback reach counters, and the first traceback
+                         * that differs from the scalar twin (TB_MISMATCH_INTS, read -1: none). */
+                        unsigned long long* aln_digest_out, int32_t* aln_count_out, int32_t* tb_reach_out,
+                        int32_t* tb_mismatch_out) {
     Params p;
     p.max_nodes = max_nodes;
     p.max_edges = poa_edge_capacity(max_nodes); /* the engine derives the edge pool from the node capacity */
@@ -241,6 +383,18 @@ void emu_polish_windows(int64_t n_windows, const int64_t* win_seq_off, const int
                 for (int32_t k = 0; k < R_FIELDS; ++k) reach[k] = 0;
             fill.reach = reach;
             fill.last_read = nullptr;
+            std::vector<unsigned long long> waln((size_t)n, 0);
+            std::vector<int32_t> walncnt((size_t)n, 0);
+            wv.aln_digest = waln.data();
+            wv.aln_count = walncnt.data();
+            std::vector<int32_t> tb_scratch(tb_reach_out ? 0 : TB_FIELDS);
+            fill.tb_reach = tb_reach_out ? tb_reach_out + w * TB_FIELDS : tb_scratch.data();
+            for (int32_t k = 0; k < TB_FIELDS; ++k) fill.tb_reach[k] = 0;
+            tb_reach_now = fill.tb_reach;
+            fill.tb_mismatch = tb_mismatch_out ? tb_mismatch_out + w * TB_MISMATCH_INTS : nullptr;
+            if (fill.tb_mismatch)
+                for (int32_t k = 0; k < TB_MISMATCH_INTS; ++k) fill.tb_mismatch[k] = -1;
+            fill.tb_last_read = nullptr;
             /* process_window writes its node count nowhere; recover it from the slot afterwards */
             uint32_t cursor = 0;
             int32_t off = 0, trim = 0;
@@ -256,6 +410,11 @@ void emu_polish_windows(int64_t n_windows, const int64_t* win_seq_off, const int
             long long moff = 0;
             int32_t mcols = 0, mst = 0;
             const int32_t n_final = process_window(s, p, wv, fill, tbs, out);
+            tb_reach_now = nullptr;
+            if (aln_digest_out)
+                for (int32_t k = 0; k < n; ++k) aln_digest_out[s0 + k] = waln[(size_t)k];
+            if (aln_count_out)
+                for (int32_t k = 0; k < n; ++k) aln_count_out[s0 + k] = walncnt[(size_t)k];
             if (digest_out)
                 for (int32_t k = 0; k < n; ++k) digest_out[s0 + k] = wdigest[(size_t)k];
             if (fill_count_out)
@@ -304,6 +463,22 @@ void emu_polish_windows(int64_t n_windows, const int64_t* win_seq_off, const int
     if (cells_out) *cells_out = total_cells.load();
     (void)rank_out;
     (void)n_nodes_out;
+}
+
+void emu_polish_windows(int64_t n_windows, const int64_t* win_seq_off, const int64_t* seq_off,
+                        const uint8_t* bases, const int8_t* weights, const uint8_t* has_weights,
+                        const int32_t* begins, const int32_t* ends, const int32_t* order, int32_t m, int32_t x, int32_t gap,
+                        int32_t max_nodes, int32_t max_edges, int32_t max_len, int32_t band_width,
+                        int32_t serial_topsort, int32_t n_threads, uint8_t* cons_out,
+                        uint16_t* cov_out, int32_t stride_out, int32_t* cons_len, int32_t* status,
+                        int32_t* rank_out, int32_t* n_nodes_out, int64_t* cells_out, int32_t* trim_out,
+                        uint8_t* msa_out, int64_t msa_cap, int64_t* msa_off, int32_t* msa_cols, int32_t* msa_status,
+                        int32_t ring_rows, unsigned long long* digest_out, int32_t* fill_count_out, int32_t* reach_out) {
+    emu_polish_windows_tb(n_windows, win_seq_off, seq_off, bases, weights, has_weights, begins, ends, order, m, x, gap,
+                          max_nodes, max_edges, max_len, band_width, serial_topsort, n_threads, cons_out, cov_out,
+                          stride_out, cons_len, status, rank_out, n_nodes_out, cells_out, trim_out, msa_out, msa_cap,
+                          msa_off, msa_cols, msa_status, ring_rows, digest_out, fill_count_out, reach_out, nullptr,
+                          nullptr, nullptr, nullptr);
 }
 
 } // extern "C"

@@ -15,6 +15,12 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 REACH_FIELDS = ("wide1", "wide2", "wide3", "wide4", "chunked_full", "fullw", "chunked_banded", "cells32",
                 "general_rows", "far_preds", "jump_preds", "max_npred", "rows_over32", "dyn_rows", "dyn_builds",
                 "retries", "retries_full", "max_len")
+#: per-window reach counters of the emulated traceback (enum TbReach in tests/emu/emu_poa.cpp), in order
+TB_REACH_FIELDS = ("tracebacks", "tile_loads", "reanchors", "global_npred", "global_pred_cap", "global_far",
+                   "common_steps", "tile_steps", "neg_chunk_steps", "band_hits", "row0_tail32", "row0_tail64", "vrun32",
+                   "count_mod0", "count_mod1", "count_mod31", "i32_reads", "partial_reads", "twin_mismatches")
+#: the first traceback of a window that differs from the scalar twin (read -1: none), in order
+TB_MISMATCH_FIELDS = ("read", "try", "entry", "twin_node", "twin_pos", "node", "pos", "twin_count", "count")
 
 
 class Emu:
@@ -28,7 +34,10 @@ class Emu:
         """Untrimmed consensus, coverage, status and DP cell count of the emulated engine.  Also kept: per sequence
         (ADD order index of the window's first sequence + processing position) the fill digest and fill count
         (last_digest, last_fill_count), per window the reach counters (last_reach: dict REACH_FIELDS -> array).
-        ring_rows: the GPU launch's score-row ring, which decides the row program's far-predecessor flags."""
+        ring_rows: the GPU launch's score-row ring, which decides the row program's far-predecessor flags.
+        Also per sequence the digest and entry count of the alignment added to the graph (last_aln_digest,
+        last_aln_count), per window the traceback's reach counters (last_tb_reach: dict TB_REACH_FIELDS -> array) and
+        its first difference from the scalar twin walk (last_tb_mismatch: W x TB_MISMATCH_FIELDS, read -1: none)."""
         W = b.n_windows
         cons = np.zeros((W, stride), dtype=np.uint8)
         cov = np.zeros((W, stride), dtype=np.uint16)
@@ -39,16 +48,23 @@ class Emu:
         self.last_digest = np.zeros(b.n_seqs, dtype=np.uint64)
         self.last_fill_count = np.zeros(b.n_seqs, dtype=np.int32)
         reach = np.zeros((W, len(REACH_FIELDS)), dtype=np.int32)
+        self.last_aln_digest = np.zeros(b.n_seqs, dtype=np.uint64)
+        self.last_aln_count = np.zeros(b.n_seqs, dtype=np.int32)
+        tb_reach = np.zeros((W, len(TB_REACH_FIELDS)), dtype=np.int32)
+        self.last_tb_mismatch = np.full((W, len(TB_MISMATCH_FIELDS)), -1, dtype=np.int32)
         order = np.ascontiguousarray(order, dtype=np.int32)
         a = _flat_args(b)
-        self.lib.emu_polish_windows(
+        self.lib.emu_polish_windows_tb(
             a[0], a[1], a[2], a[3], a[4], a[5], a[6], a[7], _p(order, C.c_int32), C.c_int32(m), C.c_int32(x), C.c_int32(g),
             C.c_int32(max_nodes), C.c_int32(max_edges), C.c_int32(max_len), C.c_int32(band),
             C.c_int32(int(serial_topsort)), C.c_int32(threads), _p(cons, C.c_uint8), _p(cov, C.c_uint16),
             C.c_int32(stride), _p(clen, C.c_int32), _p(st, C.c_int32), None, None, C.byref(cells),
             _p(self.last_trim, C.c_int32), *self._msa_args(W, msa_cap), C.c_int32(ring_rows),
-            _p(self.last_digest, C.c_uint64), _p(self.last_fill_count, C.c_int32), _p(reach, C.c_int32))
+            _p(self.last_digest, C.c_uint64), _p(self.last_fill_count, C.c_int32), _p(reach, C.c_int32),
+            _p(self.last_aln_digest, C.c_uint64), _p(self.last_aln_count, C.c_int32), _p(tb_reach, C.c_int32),
+            _p(self.last_tb_mismatch, C.c_int32))
         self.last_reach = {k: reach[:, i].copy() for i, k in enumerate(REACH_FIELDS)}
+        self.last_tb_reach = {k: tb_reach[:, i].copy() for i, k in enumerate(TB_REACH_FIELDS)}
         self.last_msa = None
         if msa_cap:  # per window: list of rows (processing order), or the status when the MSA failed
             arena, off, cols, mst = self._msa

@@ -275,7 +275,9 @@ def emu_run(emu, r, ring_rows: int, msa: bool = True):
                                   band=band, stride=2 * r["msz"], msa_cap=msa_capacity(b, r["msz"]) if msa else 0,
                                   ring_rows=ring_rows)
     return {"status": st, "cons": cons, "cov": cov, "msa": emu.last_msa, "digest": emu.last_digest.copy(),
-            "count": emu.last_fill_count.copy(), "reach": emu.last_reach}
+            "count": emu.last_fill_count.copy(), "reach": emu.last_reach, "aln_digest": emu.last_aln_digest.copy(),
+            "aln_count": emu.last_aln_count.copy(), "tb_reach": emu.last_tb_reach,
+            "tb_mismatch": emu.last_tb_mismatch.copy()}
 
 
 def ring_rows_of(r) -> int:
@@ -422,6 +424,12 @@ def _gpu_job(r):
                                                C.byref(rr), C.byref(rs))
             assert st == api.SUCCESS, api.status_string(st)
             out.update(digest=dg, count=cnt, ring_rows=rr.value, ring_stride=rs.value)
+            adg = np.zeros(b.n_seqs, dtype=np.uint64)
+            acnt = np.zeros(b.n_seqs, dtype=np.int32)
+            st = lib.b200poa_debug_aln_digest(pb.handle, adg.ctypes.data_as(C.POINTER(C.c_uint64)),
+                                              acnt.ctypes.data_as(C.POINTER(C.c_int32)), C.c_int64(b.n_seqs))
+            assert st == api.SUCCESS, api.status_string(st)
+            out.update(aln_digest=adg, aln_count=acnt)
         pb.close()
         return out
     finally:
@@ -432,11 +440,29 @@ def _gpu_job(r):
                 os.environ[k] = v
 
 
+def aln_digest_failures(name, b, got, want, what="emulation") -> list:
+    """Per window, the first read (processing position) whose alignment digest or entry count differs."""
+    bad = []
+    for w in range(b.n_windows):
+        s0, s1 = int(b.win_seq_off[w]), int(b.win_seq_off[w + 1])
+        for k in range(s1 - s0):
+            s = s0 + k
+            if got["aln_count"][s] != want["aln_count"][s] or got["aln_digest"][s] != want["aln_digest"][s]:
+                bad.append(f"{name}: window {w} read {k}: alignment of {got['aln_count'][s]} entries digest "
+                           f"{got['aln_digest'][s]:#x}, {what} {want['aln_count'][s]} entries digest "
+                           f"{want['aln_digest'][s]:#x}")
+                break
+    return bad
+
+
 def compare(r, got, want, oracle_out=None) -> list:
     """Differences between a GPU run and the emulation (and, in full band, the oracle).  Digest mismatches name the
-    window, the read (processing position) and how many fills it took."""
+    window, the read (processing position) and how many fills it took; alignment digests (where both sides have them)
+    the read and its entry counts."""
     b = r["batch"]
     bad = []
+    if "aln_digest" in got and "aln_digest" in want:
+        bad += aln_digest_failures(r["name"], b, got, want)
     if "digest" in got:
         for w in range(b.n_windows):
             s0, s1 = int(b.win_seq_off[w]), int(b.win_seq_off[w + 1])

@@ -63,6 +63,18 @@ class Oracle:
             return out, covs, pol.astype(bool), stats
         return out, covs, pol.astype(bool)
 
+    def alignment_digests(self, batch, order: np.ndarray, m: int, x: int, g: int, threads: int = 16):
+        """Per sequence (ADD-order index of the window's first sequence + processing position): the digest and pair
+        count of the alignment spoa adds to the window's graph (poa_oracle_alignment_digests; 0, 0 for backbones)."""
+        dg = np.zeros(batch.n_seqs, dtype=np.uint64)
+        cnt = np.zeros(batch.n_seqs, dtype=np.int32)
+        order = np.ascontiguousarray(order, dtype=np.int32)
+        self.lib.poa_oracle_alignment_digests.restype = None
+        self.lib.poa_oracle_alignment_digests(*_flat_args(batch), _p(order, C.c_int32), C.c_int32(m), C.c_int32(x),
+                                              C.c_int32(g), C.c_int32(threads), _p(dg, C.c_uint64),
+                                              _p(cnt, C.c_int32))
+        return dg, cnt
+
 
 def _seq_arrays(seqs, weights):
     n = len(seqs)
