@@ -993,15 +993,8 @@ int32_t b200poa_batch_launch(b200poa_batch* b) {
     a.aln_digest = b->d_aln_digest;
     a.aln_count = b->d_aln_count;
 #endif
-    /* persistent grid: one warp per resident slot.  (Shrinking the grid so that every round of it is full --
-     * 10000 windows as 3 x 3334 instead of 2.8 x 3552 -- was measured neutral: throughput follows the number of
-     * resident warps.  B200POA_GRID_BALANCE=1 keeps the experiment available.) */
-    const int max_grid = std::max(1, std::min(std::min(b->n_slots, occ * b->sm_count), b->poa_count));
-    int grid = max_grid;
-    if (std::getenv("B200POA_GRID_BALANCE")) {
-        const int rounds = (b->poa_count + max_grid - 1) / max_grid;
-        grid = std::max(1, (b->poa_count + rounds - 1) / std::max(rounds, 1));
-    }
+    /* persistent grid: one warp per resident slot */
+    const int grid = std::max(1, std::min(std::min(b->n_slots, occ * b->sm_count), b->poa_count));
     poa_window_kernel<<<grid, 32, (size_t)b->smem_bytes, b->stream>>>(a);
     CU_TRY(cudaGetLastError());
     b->launches += 1;

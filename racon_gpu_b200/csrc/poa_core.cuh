@@ -1301,6 +1301,8 @@ struct TbScratch {           /* device: shared memory (the fill's ring area); em
     uint16_t* node;          /* [TB_ROWS]   node id of row (r_hi - k)                   */
     uint8_t* readc;          /* [TB_COLS + 8] read base under column c at c - c_lo (column c <-> read[c-1]) */
 };
+/* also the capacity mark_subgraph gets for its root array (process_window) and part of the launch's shared memory: it
+ * sets the graph size above which partial-span layers take the lane-0 path (DESIGN §4) */
 constexpr int TB_SCRATCH_BYTES = TB_ROWS * TB_COLS * 2 + TB_ROWS * 4 + (TB_ROWS + 1) * 4 + TB_PRED_CAP * 4 + TB_ROWS * 2 + TB_COLS + 8 + 28 +
                                  TB_ROWS * 4 + 32 * 4 + 4 + 16;
 
@@ -1311,7 +1313,6 @@ constexpr int TB_OFF_NODE = TB_OFF_PRED + TB_PRED_CAP * 4;
 constexpr int TB_OFF_READC = TB_OFF_NODE + TB_ROWS * 2;
 constexpr int TB_OFF_INFO = (TB_OFF_READC + TB_COLS + 8 + 3) & ~3; /* [TB_ROWS] u32: node id | predecessor tile row | letter */
 constexpr int TB_OFF_OUT = TB_OFF_INFO + TB_ROWS * 4;              /* [32] u32: buffered alignment entries */
-constexpr int TB_OFF_MBAR = (TB_OFF_OUT + 32 * 4 + 7) & ~7;        /* 8 bytes: mbarrier of the bulk tile copies (TMA variant) */
 
 struct alignas(16) Vec16 { /* 8 int16 cells moved as one 128-bit access */
     uint32_t x, y, z, w;
@@ -1341,62 +1342,17 @@ POA_FN uint32_t tile_u16(tile_addr a, int32_t i) { return *reinterpret_cast<cons
 POA_FN uint32_t tile_u8(tile_addr a, int32_t i) { return poa_smem[a + (uint32_t)i]; }
 POA_FN uint32_t tile_sa(tile_addr a) { return (uint32_t)__cvta_generic_to_shared(poa_smem) + a; } /* shared-window address */
 /* asynchronous global -> shared copies used by the tile load (LDGSTS: no register staging, all in flight);
- * destinations are shared-window addresses, like every other access to the tile */
-/* Off by default: for sm_90a, ptxas 12.9 turns the cache-hinted copy into LDGSTS instructions whose shared-address base
- * and memory descriptor are uniform registers nothing writes, and the kernel dies with an illegal instruction at the
- * first tile load (tests/test_codegen.py checks every LDGSTS descriptor is written). */
-#ifndef POA_TB_EVICT_FIRST
-#define POA_TB_EVICT_FIRST 0
-#endif
-/* score chunks are read once by the traceback: with POA_TB_EVICT_FIRST they are marked first to leave L2 */
-POA_FN uint64_t tile_stream_policy() {
-    uint64_t pol = 0;
-#if POA_TB_EVICT_FIRST
-    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
-#endif
-    return pol;
-}
-POA_FN void tile_copy16(tile_addr a, int32_t byte_off, const void* src, uint64_t pol) {
-#if POA_TB_EVICT_FIRST
-    asm volatile("cp.async.cg.shared.global.L2::cache_hint [%0], [%1], 16, %2;" ::"r"(tile_sa(a) + (uint32_t)byte_off), "l"(src), "l"(pol)
-                 : "memory");
-#else
-    (void)pol;
+ * destinations are shared-window addresses, like every other access to the tile.  The copies carry no L2 cache hint:
+ * for sm_90a, ptxas 12.9 turns the hinted form into LDGSTS instructions whose shared-address base and memory descriptor
+ * are uniform registers nothing writes, and the kernel dies with an illegal instruction at the first tile load
+ * (tests/test_codegen.py checks every LDGSTS descriptor is written). */
+POA_FN void tile_copy16(tile_addr a, int32_t byte_off, const void* src) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(tile_sa(a) + (uint32_t)byte_off), "l"(src) : "memory");
-#endif
 }
 POA_FN void tile_copy4(tile_addr a, int32_t i, const void* src) {
     asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(tile_sa(a) + 4u * (uint32_t)i), "l"(src) : "memory");
 }
 POA_FN void tile_copy_wait() { asm volatile("cp.async.wait_all;" ::: "memory"); }
-/* Bulk asynchronous copies (the TMA engine's 1-D form, cp.async.bulk) with mbarrier completion: one 64-byte request per
- * tile row that lies wholly inside its band instead of four 16-byte LDGSTS.  POA_TB_TMA selects the variant. */
-#ifndef POA_TB_TMA
-#define POA_TB_TMA 0
-#endif
-POA_FN void tile_mbar_init(tile_addr a) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(tile_sa(a)) : "memory");
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-}
-POA_FN void tile_mbar_inval(tile_addr a) { asm volatile("mbarrier.inval.shared::cta.b64 [%0];" ::"r"(tile_sa(a)) : "memory"); }
-POA_FN void tile_mbar_expect(tile_addr a, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(tile_sa(a)), "r"(bytes) : "memory");
-}
-POA_FN void tile_async_fence() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-POA_FN void tile_bulk_copy(tile_addr a, int32_t byte_off, const void* src, uint32_t bytes, tile_addr mbar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                     tile_sa(a) + (uint32_t)byte_off),
-                 "l"(__cvta_generic_to_global(src)), "r"(bytes), "r"(tile_sa(mbar))
-                 : "memory");
-}
-POA_FN bool tile_mbar_test(tile_addr a, uint32_t parity) {
-    uint32_t ok;
-    asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
-                 : "=r"(ok)
-                 : "r"(tile_sa(a)), "r"(parity)
-                 : "memory");
-    return ok != 0;
-}
 POA_FN void tile_st_u32(tile_addr a, int32_t i, uint32_t v) { *reinterpret_cast<uint32_t*>(poa_smem + a + 4u * (uint32_t)i) = v; }
 POA_FN void tile_st_u16(tile_addr a, int32_t i, uint32_t v) { *reinterpret_cast<uint16_t*>(poa_smem + a + 2u * (uint32_t)i) = (uint16_t)v; }
 POA_FN void tile_st_u8(tile_addr a, int32_t i, uint32_t v) { poa_smem[a + (uint32_t)i] = (unsigned char)v; }
@@ -1407,11 +1363,9 @@ POA_FN void tile_fill8(tile_addr a, int32_t byte_off, int32_t v) { /* 8 int16 ce
 #else
 typedef uint8_t* tile_addr;
 POA_FN tile_addr tile_base(void* p) { return reinterpret_cast<uint8_t*>(p); }
-POA_FN uint64_t tile_stream_policy() { return 0; }
-POA_FN void tile_copy16(tile_addr a, int32_t byte_off, const void* src, uint64_t) { *reinterpret_cast<Vec16*>(a + byte_off) = *reinterpret_cast<const Vec16*>(src); }
+POA_FN void tile_copy16(tile_addr a, int32_t byte_off, const void* src) { *reinterpret_cast<Vec16*>(a + byte_off) = *reinterpret_cast<const Vec16*>(src); }
 POA_FN void tile_copy4(tile_addr a, int32_t i, const void* src) { reinterpret_cast<uint32_t*>(a)[i] = *reinterpret_cast<const uint32_t*>(src); }
 POA_FN void tile_copy_wait() {}
-#define POA_TB_TMA 0
 POA_FN void tile_st_u32(tile_addr a, int32_t i, uint32_t v) { reinterpret_cast<uint32_t*>(a)[i] = v; }
 POA_FN void tile_st_u16(tile_addr a, int32_t i, uint32_t v) { reinterpret_cast<uint16_t*>(a)[i] = (uint16_t)v; }
 POA_FN void tile_st_u8(tile_addr a, int32_t i, uint32_t v) { a[i] = (uint8_t)v; }
@@ -1474,16 +1428,6 @@ POA_FN_NOINLINE int32_t traceback(const Slot& s, const Params p, WinState& st, c
     const tile_addr A_rec = A_cells + TB_OFF_REC, A_poff = A_cells + TB_OFF_POFF, A_pred = A_cells + TB_OFF_PRED,
                     A_node = A_cells + TB_OFF_NODE, A_readc = A_cells + TB_OFF_READC, A_info = A_cells + TB_OFF_INFO,
                     A_out = A_cells + TB_OFF_OUT;
-#if POA_TB_TMA
-#define POA_TB_EXIT() do { POA_SYNC(); POA_LANE0 { tile_mbar_inval(A_mbar); } POA_SYNC(); } while (0)
-    const tile_addr A_mbar = A_cells + TB_OFF_MBAR;
-    uint32_t tma_parity = 0; /* phase of the mbarrier the bulk copies complete on */
-    POA_LANE0 { tile_mbar_init(A_mbar); }
-    POA_SYNC();
-#else
-#define POA_TB_EXIT() ((void)0)
-#endif
-    const uint64_t stream_pol = tile_stream_policy();
     POA_SUB_BEGIN();
     int32_t w = cap; /* write cursor (uniform) */
     int32_t i = end_row, j = rlen; /* both laundered above */
@@ -1512,7 +1456,6 @@ POA_FN_NOINLINE int32_t traceback(const Slot& s, const Params p, WinState& st, c
     while (!(i == 0 && j == 0)) {
         if (w <= 32) { /* every step consumes one entry: a path longer than nodes + read length is lost */
             st.status = ST_TRACEBACK_LOST;
-            POA_TB_EXIT();
             return cap;
         }
         if (i == 0) { /* first row: S[0][*] == 0, only horizontal moves are left */
@@ -1532,8 +1475,7 @@ POA_FN_NOINLINE int32_t traceback(const Slot& s, const Params p, WinState& st, c
             j = 0;
             if (w < 0) {
                 st.status = ST_TRACEBACK_LOST;
-                POA_TB_EXIT();
-            return cap;
+                return cap;
             }
             break;
         }
@@ -1558,42 +1500,6 @@ POA_FN_NOINLINE int32_t traceback(const Slot& s, const Params p, WinState& st, c
              * row program) instead of read from its record, so the score chunks -- the loads that go to HBM --
              * depend on nothing; they are asynchronous global->shared copies, no registers in between.  Only
              * the predecessor entries need a second, short level (two CSR offsets, cache-resident). */
-#if POA_TB_TMA
-            /* Rows that lie wholly inside their band arrive as ONE 64-byte bulk copy each (cp.async.bulk, completion
-             * counted in bytes on an mbarrier); rows cut by a band edge keep the 16-byte copies + NEG fill below. */
-            int32_t bulk_bytes = 0;
-            {
-                PerLane<int> nb_l;
-                POA_LANES(l) {
-                    int32_t n = 0;
-#pragma unroll
-                    for (int32_t rr = 0; rr < TB_RPL; ++rr) {
-                        const int32_t row = r_hi - (l + 32 * rr);
-                        if (row < r_lo) continue;
-                        const int32_t o = c_lo - band_start(gg, row, gg.n_rows);
-                        if (o >= 0 && o + TB_COLS <= bw) ++n;
-                    }
-                    nb_l[l] = n;
-                }
-                bulk_bytes = warp_sum(nb_l) * TB_COLS * 2;
-            }
-            if (bulk_bytes > 0) {
-                tile_async_fence(); /* the tile was read through the generic proxy; the bulk copies write through the async one */
-                POA_LANE0 { tile_mbar_expect(A_mbar, (uint32_t)bulk_bytes); }
-                POA_SYNC();
-                POA_LANES(l) {
-#pragma unroll
-                    for (int32_t rr = 0; rr < TB_RPL; ++rr) {
-                        const int32_t k = l + 32 * rr;
-                        const int32_t row = r_hi - k;
-                        if (row < r_lo) continue;
-                        const int32_t o = c_lo - band_start(gg, row, gg.n_rows);
-                        if (o >= 0 && o + TB_COLS <= bw)
-                            tile_bulk_copy(A_cells, k * TB_COLS * 2, S + (size_t)row * stride + o, TB_COLS * 2, A_mbar);
-                    }
-                }
-            }
-#endif
             const int32_t lo_row = r_lo < 1 ? 1 : r_lo;
             const int32_t p_lo = (int32_t)row_poff[lo_row];                           /* uniform loads (i >= 1 here) */
             const int32_t p_hi = (int32_t)row_poff[r_hi] + rec_npred(row_rec[r_hi]);
@@ -1604,16 +1510,11 @@ POA_FN_NOINLINE int32_t traceback(const Slot& s, const Params p, WinState& st, c
                     const int32_t row = r_hi - k;
                     if (row < r_lo) continue;
                     const int32_t bs = band_start(gg, row, gg.n_rows);
-#if POA_TB_TMA
-                    const bool bulk_row = c_lo - bs >= 0 && c_lo - bs + TB_COLS <= bw; /* whole row in its band: bulk copy below */
-#else
-                    const bool bulk_row = false;
-#endif
 #pragma unroll
-                    for (int32_t q = 0; q < TB_CHUNKS && !bulk_row; ++q) {
+                    for (int32_t q = 0; q < TB_CHUNKS; ++q) {
                         const int32_t o = c_lo + 8 * q - bs; /* 8-aligned both: whole chunk in the band or out */
                         const int32_t dst = (k * TB_COLS + 8 * q) * 2; /* byte offset in the tile */
-                        if (o >= 0 && o + 8 <= bw) tile_copy16(A_cells, dst, S + (size_t)row * stride + o, stream_pol);
+                        if (o >= 0 && o + 8 <= bw) tile_copy16(A_cells, dst, S + (size_t)row * stride + o);
                         else tile_fill8(A_cells, dst, NEG);
                     }
                     if (row >= 1) {
@@ -1654,14 +1555,6 @@ POA_FN_NOINLINE int32_t traceback(const Slot& s, const Params p, WinState& st, c
                     if (l + 32 * u < TB_COLS) tile_st_u8(A_readc, l + 32 * u, rb[u]);
             }
             tile_copy_wait();
-#if POA_TB_TMA
-            if (bulk_bytes > 0) {
-                int32_t spins = 0;
-                while (!tile_mbar_test(A_mbar, tma_parity) && ++spins < (1 << 22)) {}
-                if (spins >= (1 << 22)) lost = 1; /* never expected: a copy that does not complete must not hang the device */
-                tma_parity ^= 1u;
-            }
-#endif
             POA_SYNC();
             /* digest for the serial walk: a row with ONE in-edge whose source is in the tile takes the short step */
             POA_LANES(l) {
@@ -1812,7 +1705,6 @@ POA_FN_NOINLINE int32_t traceback(const Slot& s, const Params p, WinState& st, c
         } /* general step */
         if (poa_uniform_pred(lost != 0)) {
             st.status = ST_TRACEBACK_LOST;
-            POA_TB_EXIT();
             return cap;
         }
         --w;
@@ -1826,10 +1718,8 @@ POA_FN_NOINLINE int32_t traceback(const Slot& s, const Params p, WinState& st, c
     POA_TB_FLUSH();
 #undef POA_TB_FLUSH
     POA_SYNC();
-    POA_TB_EXIT();
     return w;
 }
-#undef POA_TB_EXIT
 
 /* ------------------------------------------------------------------------------------------
  * Phase 4: add the alignment to the graph  (graph.cpp:155-272, 94-116)
@@ -2835,49 +2725,6 @@ POA_FN_NOINLINE unsigned long long aln_digest(const Slot& s_ref, const Params p,
  * full-span layers; the caller trims).  Fill is the DP-fill functor:
  *     int32_t operator()(slot, params, state, geom, read) -> end row (0 = none)
  * ---------------------------------------------------------------------------------------- */
-/* Experiment (POA_PREFETCH_GRAPH): the graph phases that follow the traceback walk the graph through chains of dependent
- * loads, each of which is served from HBM when its line has left L2 since the previous read.  Ask for the lines ahead
- * of time: one prefetch per 128-byte line of the node arrays [0, N) and edge arrays [0, E). */
-#ifndef POA_PREFETCH_GRAPH
-#define POA_PREFETCH_GRAPH 0
-#endif
-#if POA_DEVICE && POA_PREFETCH_GRAPH
-__device__ __forceinline__ void prefetch_span(const void* ptr, size_t bytes) {
-    const char* b = reinterpret_cast<const char*>(ptr);
-    for (size_t o = (size_t)(threadIdx.x & 31u) * 128u; o < bytes; o += 32u * 128u) {
-#if POA_PREFETCH_GRAPH == 2
-        asm volatile("prefetch.global.L2::evict_last [%0];" ::"l"(b + o));
-#else
-        asm volatile("prefetch.global.L2 [%0];" ::"l"(b + o));
-#endif
-    }
-}
-__device__ __noinline__ void prefetch_graph(const Slot& s, int32_t N, int32_t E) {
-    const size_t n = (size_t)N, e = (size_t)E;
-    prefetch_span(s.code, n);
-    prefetch_span(s.nin, 2 * n);
-    prefetch_span(s.nout, 2 * n);
-    prefetch_span(s.in_head, 2 * n);
-    prefetch_span(s.in_tail, 2 * n);
-    prefetch_span(s.cov, 2 * n);
-    prefetch_span(s.aln_cnt, n);
-    prefetch_span(s.aln, 2 * KA * n);
-    prefetch_span(s.root, 2 * n);
-    prefetch_span(s.lpos, 2 * n);
-    prefetch_span(s.rank_of, 2 * n);
-    prefetch_span(s.e_src, 2 * e);
-    prefetch_span(s.e_dst, 2 * e);
-    prefetch_span(s.e_next, 2 * e);
-    prefetch_span(s.e_w, 4 * e);
-    prefetch_span(s.e_ord, e);
-    prefetch_span(s.cnt, 4 * n);
-    prefetch_span(s.need, 4 * n);
-    prefetch_span(s.dirty, n);
-    prefetch_span(s.marks, n);
-    prefetch_span(s.check, n);
-}
-#endif
-
 template <class Fill>
 POA_FN int32_t process_window(const Slot& s, const Params& p, const WindowView& wv, Fill& fill, const TbScratch& tbs,
                               const WindowOut& out, PhaseTimer tm = PhaseTimer{nullptr, 0}) {
@@ -2946,9 +2793,6 @@ POA_FN int32_t process_window(const Slot& s, const Params& p, const WindowView& 
 #endif
             tm.lap(PH_FILL);
             st.band_hit = 0;
-#if POA_DEVICE && POA_PREFETCH_GRAPH && POA_PREFETCH_GRAPH != 3
-            prefetch_graph(s, poa_uniform(st.n_nodes), poa_uniform(st.n_edges));
-#endif
             if (end_row <= 0) {
                 st.status = ST_TRACEBACK_LOST;
             } else {
@@ -2976,9 +2820,6 @@ POA_FN int32_t process_window(const Slot& s, const Params& p, const WindowView& 
             }
             POA_SYNC();
         }
-#endif
-#if POA_DEVICE && POA_PREFETCH_GRAPH == 3
-        prefetch_graph(s, poa_uniform(st.n_nodes), poa_uniform(st.n_edges));
 #endif
         add_alignment(s, p, st, read, wt, wconst, len, tb);
         winstate_uniform(st);

@@ -46,14 +46,7 @@ struct PerLane {
 /* Between two phases: what one lane wrote to the workspace (plain, streaming or atomic stores) must be visible to
  * every access path the other lanes use next (cached loads, L1-bypassing asynchronous copies).  In the proven-uniform
  * build __syncwarp() is elided altogether, so the ordering is asked for explicitly, once per phase boundary. */
-#ifndef POA_PHASE_FENCE
-#define POA_PHASE_FENCE 1
-#endif
-#if POA_PHASE_FENCE
 #define POA_FENCE() __threadfence_block()
-#else
-#define POA_FENCE() ((void)0)
-#endif
 
 /* Warp-uniform control flow and the compiler (ptxas 12.9, sm_90a; tests/test_codegen.py pins it).
  *
@@ -96,7 +89,6 @@ POA_FN int warp_exscan(PerLane<int>& x) {
 POA_FN unsigned warp_ballot(const PerLane<int>& p) { return __ballot_sync(0xffffffffu, p.v != 0); }
 POA_FN int warp_max(const PerLane<int>& x) { return __reduce_max_sync(0xffffffffu, x.v); }
 POA_FN int warp_min(const PerLane<int>& x) { return __reduce_min_sync(0xffffffffu, x.v); }
-POA_FN int warp_sum(const PerLane<int>& x) { return __reduce_add_sync(0xffffffffu, x.v); }
 /* value held by lane `src` (src uniform) */
 POA_FN int warp_get(const PerLane<int>& x, int src) { return __shfl_sync(0xffffffffu, x.v, src); }
 /* make a lane-0 scalar uniform across the warp */
@@ -158,11 +150,6 @@ POA_FN int warp_min(const PerLane<int>& x) {
     for (int l = 1; l < 32; ++l)
         if (x.v[l] < m) m = x.v[l];
     return m;
-}
-POA_FN int warp_sum(const PerLane<int>& x) {
-    int s = 0;
-    for (int l = 0; l < 32; ++l) s += x.v[l];
-    return s;
 }
 POA_FN int warp_get(const PerLane<int>& x, int src) { return x.v[src]; }
 POA_FN int warp_bcast0(int x) { return x; }

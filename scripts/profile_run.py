@@ -1,4 +1,6 @@
-"""Small driver for ncu captures: stage N windows, upload once, launch the POA kernel a few times."""
+"""Stage N synthetic windows, upload once, time a few launches of the POA kernel with CUDA events, and print the phase
+cycle counters (B200POA_PHASE_TIMERS=1 in the environment) and the sub-phase cycle counters (a library built with
+-DB200POA_SUBTIMERS=1 by scripts/build_variant.sh, selected with B200POA_LIB)."""
 import argparse, os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)

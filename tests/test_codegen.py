@@ -56,8 +56,8 @@ def _uniform_regs_read_by_async_copies_are_written(sass):
 
 def test_every_async_copy_reads_uniform_registers_the_kernel_writes(sass):
     """Each LDGSTS of the traceback tile takes its memory descriptor (and possibly an address base) from uniform
-    registers; ptxas once compiled the cache-hinted form into copies reading UR0 / UR1 that nothing writes, which the
-    H100 reports as an illegal instruction at the first tile load (poa_core.cuh: POA_TB_EVICT_FIRST)."""
+    registers; ptxas 12.9 compiles the L2-cache-hinted form into copies reading UR0 / UR1 that nothing writes, which the
+    H100 reports as an illegal instruction at the first tile load (poa_core.cuh: tile_copy16, DESIGN §10)."""
     used, written = _uniform_regs_read_by_async_copies_are_written(sass)
     assert used and used <= written, sorted(used - written)
 
