@@ -417,8 +417,19 @@ static int32_t branch_completion(const poa_graph* g, int64_t* scores, int32_t* p
     return max_id;
 }
 
-/* graph.cpp:440-457 generate_consensus(dst, verbose=false) + 494-542 traverse_heaviest_bundle */
+static uint64_t consensus_digest(const poa_graph* g, const int64_t* scores, const int32_t* pred, int32_t max_id,
+                                 int64_t* overflow);
+
+/* graph.cpp:440-457 generate_consensus(dst, verbose=false) + 494-542 traverse_heaviest_bundle.  cons_digest (nullable,
+ * 2 values): consensus_digest() after the first loop and after the last branch_completion; rounds: how many
+ * branch_completion ran; overflow: scores that do not fit 32 bits. */
+static int32_t graph_consensus(poa_graph* g, char** cons, uint32_t** cov, uint64_t* cons_digest, int32_t* rounds,
+                               int64_t* overflow);
 int32_t poa_graph_consensus(poa_graph* g, char** cons, uint32_t** cov) {
+    return graph_consensus(g, cons, cov, NULL, NULL, NULL);
+}
+static int32_t graph_consensus(poa_graph* g, char** cons, uint32_t** cov, uint64_t* cons_digest, int32_t* rounds,
+                               int64_t* overflow) {
     const int32_t n = g->nn;
     const int32_t* r2n = g->rank_to_node.v;
     int32_t* pred = (int32_t*)malloc(sizeof(int32_t) * (size_t)(n + 1));
@@ -442,12 +453,18 @@ int32_t poa_graph_consensus(poa_graph* g, char** cons, uint32_t** cov) {
         if (pred[id] != -1) scores[id] += scores[pred[id]];
         if (scores[max_id] < scores[id]) max_id = id;
     }
+    if (cons_digest) cons_digest[0] = consensus_digest(g, scores, pred, max_id, overflow);
+    if (rounds) *rounds = 0;
     if (g->nodes[max_id].out.n != 0) {
         int32_t* n2r = (int32_t*)malloc(sizeof(int32_t) * (size_t)n);
         for (int32_t i = 0; i < n; ++i) n2r[r2n[i]] = i;
-        while (g->nodes[max_id].out.n != 0) max_id = branch_completion(g, scores, pred, n2r[max_id]);
+        while (g->nodes[max_id].out.n != 0) {
+            max_id = branch_completion(g, scores, pred, n2r[max_id]);
+            if (rounds) ++*rounds;
+        }
         free(n2r);
     }
+    if (cons_digest) cons_digest[1] = consensus_digest(g, scores, pred, max_id, overflow);
     int32_t* path = (int32_t*)malloc(sizeof(int32_t) * (size_t)(n + 1));
     int32_t len = 0;
     while (pred[max_id] != -1) {
@@ -544,13 +561,80 @@ static uint64_t alignment_digest(const poa_pair* aln, int32_t n) {
     return t;
 }
 
+/* The engine stores a weight or a score as int32 (poa_core.cuh Slot::e_w, c_score) where spoa keeps int64: the hashes
+ * below take the low 32 bits, as the engine's wrapping sums would hold them, and count every value that does not fit
+ * (so that a truncation shows up as a failure instead of as a silent agreement). */
+static uint32_t low32(int64_t v, int64_t* overflow) {
+    if (overflow && (v > INT32_MAX || v < INT32_MIN)) ++*overflow;
+    return (uint32_t)(uint64_t)v;
+}
+
+/* Hash of the graph, the way the engine's test build hashes its own (poa_core.cuh graph_digest): the wrapping sum over
+ * nodes v of mix64(v | letter << 16 | rank << 24 | coverage << 40) (coverage as Node::coverage counts it, by labels),
+ * for the aligned id at list position q mix64(v | q << 16 | id << 24 | 1 << 56), and for the in-edge at list position
+ * k mix64(mix64(v | k << 16 | source << 32 | 2 << 56) + weight), the weight's low 32 bits. */
+static uint64_t graph_digest(const poa_graph* g, int64_t* overflow) {
+    const uint64_t K = 0x9e3779b97f4a7c15ull;
+    int32_t* rank = (int32_t*)malloc(sizeof(int32_t) * (size_t)(g->nn + 1));
+    uint8_t* seen = (uint8_t*)malloc((size_t)g->num_sequences + 1);
+    for (int32_t r = 0; r < g->rank_to_node.n; ++r) rank[g->rank_to_node.v[r]] = r;
+    uint64_t t = 0;
+    for (int32_t v = 0; v < g->nn; ++v) {
+        const node_t* nd = &g->nodes[v];
+        t += digest_mix64(((uint64_t)v | ((uint64_t)(uint8_t)nd->letter << 16) | ((uint64_t)(uint16_t)rank[v] << 24) |
+                           ((uint64_t)(uint16_t)node_coverage(g, v, seen) << 40)) + K);
+        for (int32_t q = 0; q < nd->aligned.n; ++q)
+            t += digest_mix64(((uint64_t)v | ((uint64_t)q << 16) | ((uint64_t)nd->aligned.v[q] << 24) | (1ull << 56)) + K);
+        for (int32_t k = 0; k < nd->in.n; ++k) {
+            const edge_t* e = &g->edges[nd->in.v[k]];
+            const uint64_t h = digest_mix64(((uint64_t)v | ((uint64_t)k << 16) | ((uint64_t)e->src << 32) | (2ull << 56)) + K);
+            t += digest_mix64(h + low32(e->weight, overflow));
+        }
+    }
+    free(seen);
+    free(rank);
+    return t;
+}
+
+/* Hash of a subgraph's member order as graph ids (poa_core.cuh sub_digest): sum over k of mix64(k << 32 | id | 3 << 56) */
+static uint64_t subgraph_digest(const poa_graph* s, const int32_t* mapping) {
+    uint64_t t = 0;
+    for (int32_t k = 0; k < s->rank_to_node.n; ++k)
+        t += digest_mix64(((uint64_t)(uint16_t)mapping[s->rank_to_node.v[k]] | ((uint64_t)k << 32) | (3ull << 56)) +
+                          0x9e3779b97f4a7c15ull);
+    return t;
+}
+
+/* Hash of the consensus scores (poa_core.cuh cons_digest): sum over nodes v of mix64(mix64(v | 4 << 56) + (score |
+ * pred << 32)), both as their low 32 bits, plus mix64(max_id | 5 << 56) */
+static uint64_t consensus_digest(const poa_graph* g, const int64_t* scores, const int32_t* pred, int32_t max_id,
+                                 int64_t* overflow) {
+    const uint64_t K = 0x9e3779b97f4a7c15ull;
+    uint64_t t = digest_mix64(((uint64_t)(uint32_t)max_id | (5ull << 56)) + K);
+    for (int32_t v = 0; v < g->nn; ++v)
+        t += digest_mix64(digest_mix64(((uint64_t)v | (4ull << 56)) + K) +
+                          ((uint64_t)low32(scores[v], overflow) | ((uint64_t)(uint32_t)pred[v] << 32)));
+    return t;
+}
+
+/* per sequence of a window: what poa_oracle_graph_digests reports (all nullable) */
+typedef struct {
+    uint64_t* graph_digest;
+    int32_t* graph_nodes;
+    int32_t* graph_edges;
+    uint64_t* sub_digest;
+    int32_t* sub_count;
+    int64_t* overflow;
+} graph_trace;
+
 /* window.cpp:73-116: the graph of one window -- backbone, then every layer aligned (whole graph or subgraph) and added.
  * aln_digest / aln_count (nullable, n_seqs each): per sequence the digest and length of the alignment that was added
- * (graph ids; 0 and 0 for the backbone). */
+ * (graph ids; 0 and 0 for the backbone).  gt (nullable): per sequence the graph after it was added, and the subgraph a
+ * partial-span read was aligned to. */
 static poa_graph* window_graph(int32_t n_seqs, const char* const* seqs, const int32_t* lens,
                                const int8_t* const* weights, const int32_t* begins, const int32_t* ends,
                                int32_t m, int32_t x, int32_t gap, int64_t* stats, uint64_t* aln_digest,
-                               int32_t* aln_count) {
+                               int32_t* aln_count, const graph_trace* gt) {
     int32_t maxlen = 0;
     for (int32_t i = 0; i < n_seqs; ++i)
         if (lens[i] > maxlen) maxlen = lens[i];
@@ -561,12 +645,23 @@ static poa_graph* window_graph(int32_t n_seqs, const char* const* seqs, const in
     if (aln_count) aln_count[0] = 0;
     for (int32_t k = 0; k < lens[0]; ++k) w[k] = weights[0] ? (uint32_t)weights[0][k] : 1u;
     poa_graph_add_alignment(g, NULL, 0, seqs[0], lens[0], w); /* window.cpp:73-76 */
+    if (gt) {
+        gt->graph_digest[0] = graph_digest(g, gt->overflow);
+        gt->graph_nodes[0] = g->nn;
+        gt->graph_edges[0] = g->ne;
+        gt->sub_digest[0] = 0;
+        gt->sub_count[0] = 0;
+    }
 
     const uint32_t L = (uint32_t)lens[0];
     const uint32_t offset = (uint32_t)(0.01 * L); /* window.cpp:87 */
     for (int32_t i = 1; i < n_seqs; ++i) {
         poa_pair* aln = NULL;
         int32_t n_aln;
+        if (gt) {
+            gt->sub_digest[i] = 0;
+            gt->sub_count[i] = 0;
+        }
         if (!begins || ((uint32_t)begins[i] < offset && (uint32_t)ends[i] > L - offset)) { /* window.cpp:92-95 */
             if (stats) {
                 stats[2] += (int64_t)g->nn * (lens[i] + 1);
@@ -576,6 +671,10 @@ static poa_graph* window_graph(int32_t n_seqs, const char* const* seqs, const in
         } else { /* window.cpp:96-103 */
             int32_t* mapping = (int32_t*)malloc(sizeof(int32_t) * (size_t)(g->nn + 1));
             poa_graph* s = subgraph(g, begins[i], ends[i], mapping);
+            if (gt) {
+                gt->sub_digest[i] = subgraph_digest(s, mapping);
+                gt->sub_count[i] = s->nn;
+            }
             if (stats) {
                 stats[2] += (int64_t)s->nn * (lens[i] + 1);
                 stats[4] += (int64_t)s->nn * (lens[i] + 1 < 256 ? lens[i] + 1 : 256);
@@ -592,6 +691,11 @@ static poa_graph* window_graph(int32_t n_seqs, const char* const* seqs, const in
         poa_graph_add_alignment(g, aln, n_aln, seqs[i], lens[i], w);
         free(aln);
         if (stats) stats[3] += 1;
+        if (gt) {
+            gt->graph_digest[i] = graph_digest(g, gt->overflow);
+            gt->graph_nodes[i] = g->nn;
+            gt->graph_edges[i] = g->ne;
+        }
     }
     free(w);
     return g;
@@ -611,7 +715,7 @@ int32_t poa_oracle_window_consensus(int32_t n_seqs, const char* const* seqs, con
         if (cov_out) memset(cov_out, 0, sizeof(uint32_t) * (size_t)lens[0]);
         return lens[0];
     }
-    poa_graph* g = window_graph(n_seqs, seqs, lens, weights, begins, ends, m, x, gap, stats, NULL, NULL);
+    poa_graph* g = window_graph(n_seqs, seqs, lens, weights, begins, ends, m, x, gap, stats, NULL, NULL, NULL);
 
     char* cons = NULL;
     uint32_t* cov = NULL;
@@ -695,7 +799,7 @@ int32_t poa_oracle_window_msa(int32_t n_seqs, const char* const* seqs, const int
                               const int8_t* const* weights, const int32_t* begins, const int32_t* ends,
                               int32_t m, int32_t x, int32_t gap, char** rows_out, int32_t* msa_len) {
     if (!ends) begins = NULL;
-    poa_graph* g = window_graph(n_seqs, seqs, lens, weights, begins, ends, m, x, gap, NULL, NULL, NULL);
+    poa_graph* g = window_graph(n_seqs, seqs, lens, weights, begins, ends, m, x, gap, NULL, NULL, NULL, NULL);
     int32_t n = poa_graph_msa(g, rows_out, msa_len);
     poa_graph_destroy(g);
     return n;
@@ -728,6 +832,11 @@ typedef struct {
     int64_t* stats;
     uint64_t* aln_digest; /* set: the job digests alignments (poa_oracle_alignment_digests) instead of polishing */
     int32_t* aln_count;
+    graph_trace graph;    /* graph.graph_digest set: the job digests graphs (poa_oracle_graph_digests) */
+    uint64_t* cons_digest;
+    int32_t* cons_rounds;
+    int64_t* overflow;    /* [n_windows] */
+    int32_t* max_indegree; /* [n_windows] */
     int64_t cursor;
     pthread_mutex_t mu;
 } batch_job;
@@ -765,7 +874,26 @@ static void* batch_worker(void* arg) {
         }
         if (job->aln_digest) {
             poa_graph_destroy(window_graph(n, seqs, lens, wts, bg, en, job->m, job->x, job->gap, NULL,
-                                           job->aln_digest + s0, job->aln_count + s0));
+                                           job->aln_digest + s0, job->aln_count + s0, NULL));
+            continue;
+        }
+        if (job->graph.graph_digest) {
+            int64_t* of = job->overflow + w;
+            *of = 0;
+            const graph_trace gt = {job->graph.graph_digest + s0, job->graph.graph_nodes + s0,
+                                    job->graph.graph_edges + s0, job->graph.sub_digest + s0, job->graph.sub_count + s0,
+                                    of};
+            poa_graph* g = window_graph(n, seqs, lens, wts, bg, en, job->m, job->x, job->gap, NULL, NULL, NULL, &gt);
+            int32_t deg = 0;
+            for (int32_t v = 0; v < g->nn; ++v)
+                if (g->nodes[v].in.n > deg) deg = g->nodes[v].in.n;
+            job->max_indegree[w] = deg;
+            char* cons = NULL;
+            uint32_t* ccov = NULL;
+            graph_consensus(g, &cons, &ccov, job->cons_digest + 2 * w, job->cons_rounds + w, of);
+            free(cons);
+            free(ccov);
+            poa_graph_destroy(g);
             continue;
         }
         int32_t pol = 0;
@@ -821,6 +949,38 @@ void poa_oracle_alignment_digests(int64_t n_windows, const int64_t* win_seq_off,
     job.gap = gap;
     job.aln_digest = aln_digest;
     job.aln_count = aln_count;
+    run_batch_job(&job, n_threads);
+}
+
+void poa_oracle_graph_digests(int64_t n_windows, const int64_t* win_seq_off, const int64_t* seq_off,
+                              const uint8_t* bases, const int8_t* weights, const uint8_t* has_weights,
+                              const int32_t* begins, const int32_t* ends, const int32_t* order, int32_t m, int32_t x,
+                              int32_t gap, int32_t n_threads, uint64_t* graph_digest, int32_t* graph_nodes,
+                              int32_t* graph_edges, uint64_t* sub_digest, int32_t* sub_count, uint64_t* cons_digest,
+                              int32_t* cons_rounds, int64_t* overflow, int32_t* max_indegree) {
+    batch_job job;
+    memset(&job, 0, sizeof(job));
+    job.n_windows = n_windows;
+    job.win_seq_off = win_seq_off;
+    job.seq_off = seq_off;
+    job.bases = bases;
+    job.weights = weights;
+    job.has_weights = has_weights;
+    job.begins = begins;
+    job.ends = ends;
+    job.order = order;
+    job.m = m;
+    job.x = x;
+    job.gap = gap;
+    job.graph.graph_digest = graph_digest;
+    job.graph.graph_nodes = graph_nodes;
+    job.graph.graph_edges = graph_edges;
+    job.graph.sub_digest = sub_digest;
+    job.graph.sub_count = sub_count;
+    job.cons_digest = cons_digest;
+    job.cons_rounds = cons_rounds;
+    job.overflow = overflow;
+    job.max_indegree = max_indegree;
     run_batch_job(&job, n_threads);
 }
 

@@ -98,6 +98,20 @@ void poa_oracle_alignment_digests(int64_t n_windows, const int64_t* win_seq_off,
                                   const int32_t* begins, const int32_t* ends, const int32_t* order, int32_t m,
                                   int32_t x, int32_t gap, int32_t n_threads, uint64_t* aln_digest, int32_t* aln_count);
 
+/* spoa's graph of each window, hashed the way the engine's test build hashes its own (poa_core.cuh graph_digest,
+ * sub_digest, cons_digest); same flat layout and processing order as poa_oracle_alignment_digests.  Per sequence: the
+ * graph after it was added (the backbone: after the chain) with its node and edge counts, and for a partial-span read
+ * the member order of the subgraph it was aligned to (graph ids) with the member count (else 0 and 0).  Per window:
+ * the consensus scores after traverse_heaviest_bundle's first loop and after the last branch_completion (2 values),
+ * the number of branch_completion rounds, how many weights or scores did not fit 32 bits (the engine keeps them as
+ * int32; the hashes take the low 32 bits), and the largest in-degree of the final graph. */
+void poa_oracle_graph_digests(int64_t n_windows, const int64_t* win_seq_off, const int64_t* seq_off,
+                              const uint8_t* bases, const int8_t* weights, const uint8_t* has_weights,
+                              const int32_t* begins, const int32_t* ends, const int32_t* order, int32_t m, int32_t x,
+                              int32_t gap, int32_t n_threads, uint64_t* graph_digest, int32_t* graph_nodes,
+                              int32_t* graph_edges, uint64_t* sub_digest, int32_t* sub_count, uint64_t* cons_digest,
+                              int32_t* cons_rounds, int64_t* overflow, int32_t* max_indegree);
+
 /* spoa::Graph::generate_multiple_sequence_alignment(dst, false)  (graph.cpp:373-427): one row per sequence in the
  * order they were added, '-' where the sequence has no base in a column.  *rows_out is one malloc'ed block of
  * n_rows x *msa_len bytes (free with poa_oracle_free); returns n_rows. */

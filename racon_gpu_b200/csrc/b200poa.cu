@@ -76,6 +76,15 @@ struct KernelArgs {
     unsigned long long* aln_digest;  /* [staged sequences] see b200poa_debug_aln_digest */
     int32_t* aln_count;
 #endif
+#if POA_GRAPH_DIGEST
+    unsigned long long* graph_digest; /* [staged sequences] see b200poa_debug_graph_digest */
+    int32_t* graph_nodes;
+    int32_t* graph_edges;
+    unsigned long long* sub_digest;
+    int32_t* sub_count;
+    unsigned long long* cons_digest;  /* [2 x staged windows] */
+    int32_t* cons_rounds;             /* [staged windows] */
+#endif
 };
 
 #ifndef POA_MIN_BLOCKS_PER_SM
@@ -137,6 +146,13 @@ __global__ void __launch_bounds__(32, POA_MIN_BLOCKS_PER_SM) poa_window_kernel(c
         wv.aln_digest = a.aln_digest + s0;
         wv.aln_count = a.aln_count + s0;
 #endif
+#if POA_GRAPH_DIGEST
+        wv.graph_digest = a.graph_digest + s0;
+        wv.graph_nodes = a.graph_nodes + s0;
+        wv.graph_edges = a.graph_edges + s0;
+        wv.sub_digest = a.sub_digest + s0;
+        wv.sub_count = a.sub_count + s0;
+#endif
         WindowOut out;
         out.cons = a.out_cons;
         out.cov = a.out_cov;
@@ -146,6 +162,10 @@ __global__ void __launch_bounds__(32, POA_MIN_BLOCKS_PER_SM) poa_window_kernel(c
         out.off = a.out_off + w;
         out.trim = a.out_trim + w;
         out.trim_nseq = a.win_trim_nseq[w];
+#if POA_GRAPH_DIGEST
+        out.cons_digest = a.cons_digest + 2 * (size_t)w;
+        out.cons_rounds = a.cons_rounds + w;
+#endif
         const int32_t n_nodes = poa_uniform(process_window(s, a.p, wv, fill, tbs, out, PhaseTimer{a.phase_cycles, 0}));
         if (a.out_msa) { /* B200POA_OUTPUT_MSA */
             MsaOut mo;
@@ -274,6 +294,15 @@ struct b200poa_batch {
     unsigned long long* d_aln_digest = nullptr; /* [max_seqs] see b200poa_debug_aln_digest */
     int32_t* d_aln_count = nullptr;
 #endif
+#if POA_GRAPH_DIGEST
+    unsigned long long* d_graph_digest = nullptr; /* [max_seqs] see b200poa_debug_graph_digest */
+    int32_t* d_graph_nodes = nullptr;
+    int32_t* d_graph_edges = nullptr;
+    unsigned long long* d_sub_digest = nullptr;
+    int32_t* d_sub_count = nullptr;
+    unsigned long long* d_cons_digest = nullptr; /* [2 x max_poas] */
+    int32_t* d_cons_rounds = nullptr;            /* [max_poas] */
+#endif
     size_t msa_cap = 0;
     size_t msa_bound = 0;                  /* worst-case MSA bytes of the windows staged so far */
     bool msa_fetched = false;
@@ -393,6 +422,15 @@ static void free_batch(b200poa_batch* b) {
 #if POA_ALN_DIGEST
     cudaFree(b->d_aln_digest);
     cudaFree(b->d_aln_count);
+#endif
+#if POA_GRAPH_DIGEST
+    cudaFree(b->d_graph_digest);
+    cudaFree(b->d_graph_nodes);
+    cudaFree(b->d_graph_edges);
+    cudaFree(b->d_sub_digest);
+    cudaFree(b->d_sub_count);
+    cudaFree(b->d_cons_digest);
+    cudaFree(b->d_cons_rounds);
 #endif
     delete b;
 }
@@ -598,6 +636,15 @@ static int32_t alloc_batch_memory(b200poa_batch* b) {
 #if POA_ALN_DIGEST
     CU_TRY(cudaMalloc(&b->d_aln_digest, (MS + 1) * sizeof(unsigned long long)));
     CU_TRY(cudaMalloc(&b->d_aln_count, (MS + 1) * sizeof(int32_t)));
+#endif
+#if POA_GRAPH_DIGEST
+    CU_TRY(cudaMalloc(&b->d_graph_digest, (MS + 1) * sizeof(unsigned long long)));
+    CU_TRY(cudaMalloc(&b->d_graph_nodes, (MS + 1) * sizeof(int32_t)));
+    CU_TRY(cudaMalloc(&b->d_graph_edges, (MS + 1) * sizeof(int32_t)));
+    CU_TRY(cudaMalloc(&b->d_sub_digest, (MS + 1) * sizeof(unsigned long long)));
+    CU_TRY(cudaMalloc(&b->d_sub_count, (MS + 1) * sizeof(int32_t)));
+    CU_TRY(cudaMalloc(&b->d_cons_digest, 2 * (MP + 1) * sizeof(unsigned long long)));
+    CU_TRY(cudaMalloc(&b->d_cons_rounds, (MP + 1) * sizeof(int32_t)));
 #endif
     return B200POA_SUCCESS;
 }
@@ -993,6 +1040,25 @@ int32_t b200poa_batch_launch(b200poa_batch* b) {
     a.aln_digest = b->d_aln_digest;
     a.aln_count = b->d_aln_count;
 #endif
+#if POA_GRAPH_DIGEST
+    {
+        const size_t ns = (size_t)b->seq_count, nw = (size_t)b->poa_count;
+        CU_TRY(cudaMemsetAsync(b->d_graph_digest, 0, ns * sizeof(unsigned long long), b->stream));
+        CU_TRY(cudaMemsetAsync(b->d_graph_nodes, 0, ns * sizeof(int32_t), b->stream));
+        CU_TRY(cudaMemsetAsync(b->d_graph_edges, 0, ns * sizeof(int32_t), b->stream));
+        CU_TRY(cudaMemsetAsync(b->d_sub_digest, 0, ns * sizeof(unsigned long long), b->stream));
+        CU_TRY(cudaMemsetAsync(b->d_sub_count, 0, ns * sizeof(int32_t), b->stream));
+        CU_TRY(cudaMemsetAsync(b->d_cons_digest, 0, 2 * nw * sizeof(unsigned long long), b->stream));
+        CU_TRY(cudaMemsetAsync(b->d_cons_rounds, 0, nw * sizeof(int32_t), b->stream));
+    }
+    a.graph_digest = b->d_graph_digest;
+    a.graph_nodes = b->d_graph_nodes;
+    a.graph_edges = b->d_graph_edges;
+    a.sub_digest = b->d_sub_digest;
+    a.sub_count = b->d_sub_count;
+    a.cons_digest = b->d_cons_digest;
+    a.cons_rounds = b->d_cons_rounds;
+#endif
     /* persistent grid: one warp per resident slot */
     const int grid = std::max(1, std::min(std::min(b->n_slots, occ * b->sm_count), b->poa_count));
     poa_window_kernel<<<grid, 32, (size_t)b->smem_bytes, b->stream>>>(a);
@@ -1181,6 +1247,31 @@ extern "C" int32_t b200poa_debug_aln_digest(b200poa_batch* b, uint64_t* digest, 
     CU_TRY(cudaStreamSynchronize(b->stream));
     CU_TRY(cudaMemcpy(digest, b->d_aln_digest, (size_t)b->seq_count * sizeof(uint64_t), cudaMemcpyDeviceToHost));
     CU_TRY(cudaMemcpy(count, b->d_aln_count, (size_t)b->seq_count * sizeof(int32_t), cudaMemcpyDeviceToHost));
+    return B200POA_SUCCESS;
+}
+#endif
+#if POA_GRAPH_DIGEST
+/* test build only: after the last launch, per staged sequence (same order as b200poa_debug_fill_digest) graph_digest()
+ * of the graph after the sequence was added and sorted with its node and edge counts (0 once its window stopped on a
+ * status), and for partial-span reads sub_digest() of the subgraph's member order with its member count (else 0 and 0);
+ * per staged window (add order) cons_digest() after the full scoring pass and after the last round of branch
+ * completion, and the number of rounds (0 where no consensus was generated).  Synchronises. */
+extern "C" int32_t b200poa_debug_graph_digest(b200poa_batch* b, uint64_t* graph_digest, int32_t* graph_nodes,
+                                              int32_t* graph_edges, uint64_t* sub_digest, int32_t* sub_count, int64_t n,
+                                              uint64_t* cons_digest, int32_t* cons_rounds, int64_t n_windows) {
+    if (!b || !graph_digest || !graph_nodes || !graph_edges || !sub_digest || !sub_count || !cons_digest ||
+        !cons_rounds || n < b->seq_count || n_windows < b->poa_count)
+        return B200POA_INVALID_ARGUMENT;
+    DeviceGuard g(b->device);
+    CU_TRY(cudaStreamSynchronize(b->stream));
+    const size_t ns = (size_t)b->seq_count, nw = (size_t)b->poa_count;
+    CU_TRY(cudaMemcpy(graph_digest, b->d_graph_digest, ns * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+    CU_TRY(cudaMemcpy(graph_nodes, b->d_graph_nodes, ns * sizeof(int32_t), cudaMemcpyDeviceToHost));
+    CU_TRY(cudaMemcpy(graph_edges, b->d_graph_edges, ns * sizeof(int32_t), cudaMemcpyDeviceToHost));
+    CU_TRY(cudaMemcpy(sub_digest, b->d_sub_digest, ns * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+    CU_TRY(cudaMemcpy(sub_count, b->d_sub_count, ns * sizeof(int32_t), cudaMemcpyDeviceToHost));
+    CU_TRY(cudaMemcpy(cons_digest, b->d_cons_digest, 2 * nw * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+    CU_TRY(cudaMemcpy(cons_rounds, b->d_cons_rounds, nw * sizeof(int32_t), cudaMemcpyDeviceToHost));
     return B200POA_SUCCESS;
 }
 #endif

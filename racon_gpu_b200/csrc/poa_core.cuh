@@ -51,6 +51,13 @@
 #ifndef POA_ALN_DIGEST
 #define POA_ALN_DIGEST 0
 #endif
+/* Test build (-DPOA_GRAPH_DIGEST=1, the same library and tests/emu): the graph after every read (graph_digest), the
+ * subgraph a partial-span read is aligned to (sub_digest) and the consensus scores before and after branch completion
+ * (cons_digest) are hashed, so that add_alignment, the sorts, the subgraph and the heaviest bundle can be compared read
+ * for read with the emulation and with spoa.  A define of its own, like POA_ALN_DIGEST. */
+#ifndef POA_GRAPH_DIGEST
+#define POA_GRAPH_DIGEST 0
+#endif
 
 /* Hooks of the emulation (tests/emu): POA_TB_REACH(field) counts a path of the traceback, POA_TB_REACH_IF(cond, field)
  * counts it when cond holds, and POA_TB_TWIN(fill, ...) checks every traceback against a scalar twin walk.  Elsewhere
@@ -63,6 +70,21 @@
 #endif
 #ifndef POA_TB_TWIN
 #define POA_TB_TWIN(fill, ...) ((void)0)
+#endif
+/* The same for the graph phases: POA_GRAPH_REACH(field) / POA_GRAPH_REACH_IF(cond, field) count a path of
+ * add_alignment, the sorts, the subgraph or the consensus, and POA_GRAPH_TWIN(what, ...) checks the sort, the subgraph
+ * and the consensus scores against their serial twins.  Elsewhere nothing. */
+#ifndef POA_GRAPH_REACH
+#define POA_GRAPH_REACH(field) ((void)0)
+#endif
+#ifndef POA_GRAPH_REACH_IF
+#define POA_GRAPH_REACH_IF(cond, field) ((void)0)
+#endif
+#ifndef POA_GRAPH_REACH_AT /* the k-th of the counters that start at field */
+#define POA_GRAPH_REACH_AT(field, k) ((void)0)
+#endif
+#ifndef POA_GRAPH_TWIN
+#define POA_GRAPH_TWIN(what, ...) ((void)0)
 #endif
 
 namespace b200poa {
@@ -273,6 +295,14 @@ struct WindowView {
                                         (last adaptive try) */
     int32_t* aln_count;              /* [n_seqs] its entries */
 #endif
+#if POA_GRAPH_DIGEST
+    unsigned long long* graph_digest; /* [n_seqs] test build only: graph_digest() after sequence r was added and sorted
+                                         (r = 0: the backbone); 0 once the window stopped on a status */
+    int32_t* graph_nodes;             /* [n_seqs] nodes and edges of that graph */
+    int32_t* graph_edges;
+    unsigned long long* sub_digest;   /* [n_seqs] partial-span reads: sub_digest() of the subgraph's member order */
+    int32_t* sub_count;               /* [n_seqs] its members */
+#endif
 };
 
 /* Where a window's result goes: consensus and coverage are appended to compact arenas (one bump allocation per
@@ -288,6 +318,11 @@ struct WindowOut {
     int32_t* trim;     /* ... first (low 16 bits) and last (high 16 bits, signed) index whose coverage is
                           >= (trim_nseq - 1) / 2; first > last: no such base */
     int32_t trim_nseq; /* sequences the trim threshold counts (window.cpp:121: sequences_.size()) */
+#if POA_GRAPH_DIGEST
+    unsigned long long* cons_digest; /* [2] test build only: cons_digest() after consensus_scores_full() and after the
+                                        last round of branch completion (generate_consensus writes them) */
+    int32_t* cons_rounds;            /* rounds of branch completion */
+#endif
 };
 
 /* OutputType::msa: a window's rows are bump-allocated in a compact arena like its consensus (n_seqs rows of `cols`
@@ -816,6 +851,7 @@ POA_FN_NOINLINE void subgraph_members(const Slot& s_ref, int32_t N, int32_t begi
     POA_SYNC();
     /* ---- members and their sroot ---- */
     for (int32_t hi = r_top; hi >= 0; hi -= 32 - (KA + 1)) {
+        POA_GRAPH_TWIN(sweep_chunk, s, hi);
         /* the chunk's topology, read once: up to four in-edge sources and the aligned nodes of every lane's node, packed
          * two ids per register (a longer in-edge list is walked in memory each time its node has something to pass on) */
         PerLane<int> vv, n_src, passed, s01, s23, m01, m23, m45, m6;
@@ -889,6 +925,7 @@ POA_FN_NOINLINE void subgraph_members(const Slot& s_ref, int32_t N, int32_t begi
                 else passed[l] = x;   /* every target already holds it */
             }
             POA_SYNC();
+            POA_GRAPH_TWIN(sweep_step);
             if (!warp_ballot(ch)) break;
         }
         if (hi < 32) break; /* this chunk reached rank 0 */
@@ -1045,6 +1082,7 @@ POA_FN_NOINLINE int32_t subgraph_order(const Slot& s_ref, int32_t N, const uint1
 POA_FN int32_t mark_subgraph(const Slot& s, const Params& p, WinState& st, int32_t begin, int32_t end, uint16_t* sroot,
                              int32_t sroot_cap) {
     const int32_t N = poa_uniform(st.n_nodes);
+    POA_GRAPH_REACH_IF(!p.serial_topsort && N > sroot_cap, sub_serial);
     if (p.serial_topsort || N > sroot_cap) return mark_subgraph_serial(s, p, st, begin, end);
     subgraph_members(s, N, begin, end, sroot);
     return subgraph_order(s, N, sroot);
@@ -1767,6 +1805,7 @@ POA_FN_NOINLINE void add_alignment(const Slot& s_ref, const Params p_ref, WinSta
                             break;
                         }
                     }
+                    POA_GRAPH_REACH_IF(a >= 0, clique_mate);
                 }
                 s.asg[pos] = a;
             }
@@ -1821,6 +1860,7 @@ POA_FN_NOINLINE void add_alignment(const Slot& s_ref, const Params p_ref, WinSta
                 if (na + 1 > KA) {
                     bad[l] = 1;
                 } else {
+                    POA_GRAPH_REACH_AT(join1, na);
                     for (int32_t q = 0; q < na; ++q) {
                         const int32_t y = s.aln[x * KA + q];
                         s.aln[v * KA + q] = (uint16_t)y;
@@ -1847,6 +1887,8 @@ POA_FN_NOINLINE void add_alignment(const Slot& s_ref, const Params p_ref, WinSta
         st.status = fail;
         return;
     }
+    POA_GRAPH_REACH_IF(n_new >= 32, new_nodes32);
+    POA_GRAPH_REACH_IF(n_new >= 64, new_nodes64);
 
     POA_SUB_LAP(3);
     /* (c) roots of new unaligned nodes: root[v] = min(v, root[next node on the read path]); a run
@@ -1872,6 +1914,7 @@ POA_FN_NOINLINE void add_alignment(const Slot& s_ref, const Params p_ref, WinSta
                 if ((int32_t)s.root[u] < r) r = s.root[u];
                 break;
             }
+            POA_GRAPH_REACH_IF((q >> 5) != (pos >> 5), run_cross32);
             s.roff[v] = (uint32_t)r; /* stage: root[] of run members is still NONE16 for the others */
         }
     }
@@ -1918,7 +1961,12 @@ POA_FN_NOINLINE void add_alignment_edges(const Slot& s_ref, const Params p_ref, 
 #define POA_ADD_DU 4
 #endif
     constexpr int DU = POA_ADD_DU;
+    POA_GRAPH_REACH_IF(len == 1, read_len1);
+    POA_GRAPH_REACH_IF(wt == nullptr, const_weights);
+    POA_GRAPH_REACH_IF(wt != nullptr, base_weights);
+    POA_GRAPH_REACH_IF(wt == nullptr && wconst == 0, weight0);
     for (int32_t base = 0; base < len; base += 32 * DU) {
+        POA_GRAPH_REACH_IF(base + 32 * (DU - 1) < len, du_all);
         PerLane<int> hit[DU], need[DU];
         POA_LANES(l) {
             int32_t cur[DU], prev[DU], f[DU];
@@ -1969,6 +2017,8 @@ POA_FN_NOINLINE void add_alignment_edges(const Slot& s_ref, const Params p_ref, 
                 const int32_t pos = base + 32 * u + l;
                 hit[u][l] = f[u];
                 need[u][l] = (pos < len && pos > 0 && f[u] < 0) ? 1 : 0;
+                POA_GRAPH_REACH_IF(pos < len && pos > 0 && (f[u] >= 0 ? s.e_ord[f[u]] >= 32 : s.nin[cur[u]] > 32),
+                                   walk_over32);
             }
         }
         unsigned nmask[DU];
@@ -2011,9 +2061,14 @@ POA_FN_NOINLINE void add_alignment_edges(const Slot& s_ref, const Params p_ref, 
             for (int32_t u = 0; u < DU; ++u) {
                 if (!act[u]) continue;
                 const int32_t h = hit[u][l];
+                POA_GRAPH_REACH_IF(wt != nullptr && wt[base + 32 * u + l] == 0, weight0);
                 if (h >= 0) {
+                    POA_GRAPH_REACH(edge_bumped);
                     s.e_w[h] = old_w[u] + w[u];
                 } else {
+                    POA_GRAPH_REACH(edge_created);
+                    POA_GRAPH_REACH_IF(root_p[u] == root_c[u], edge_same_root);
+                    POA_GRAPH_REACH_IF(root_p[u] != root_c[u], edge_cross_root);
                     const int32_t e = n_edges + first[u] + poa_popc(nmask[u] & ((1u << l) - 1u));
                     s.e_src[e] = (uint16_t)prev[u];
                     s.e_dst[e] = (uint16_t)cur[u];
@@ -2213,6 +2268,7 @@ POA_FN_NOINLINE void topsort_roots(const Slot& s_ref, const Params p_ref, WinSta
     }
     POA_SYNC();
     POA_SUB_LAP(7);
+    POA_GRAPH_REACH_IF(n_work > 32, dirty_over32);
     /* 2b. spoa's DFS restricted to the members of each dirty root, 32 roots at a time */
     for (int32_t base = 0; base < n_work; base += 32) {
         POA_LANES(l) {
@@ -2381,10 +2437,13 @@ POA_FN void consensus_scores_full(const Slot& s, int32_t N, int32_t& max_id_out)
                         const int32_t u = s.e_src[e];
                         const int32_t ww = s.e_w[e];
                         if (sc < ww || (sc == ww && s.c_score[best] <= s.c_score[u])) {
+                            POA_GRAPH_REACH_IF(sc == ww && s.c_score[best] == s.c_score[u], tie_equal_pred);
                             sc = ww;
                             best = u;
                         }
                     }
+                    POA_GRAPH_REACH_IF(best != -1 && (int32_t)s.rank_of[best] >= r0, tie_in_block);
+                    POA_GRAPH_REACH_IF(best != -1 && (int32_t)s.rank_of[best] < r0, tie_pre_block);
                     if (best != -1) sc += s.c_score[best];
                     score[l] = sc;
                     s.c_score[v] = sc;
@@ -2411,12 +2470,19 @@ POA_FN void consensus_scores_full(const Slot& s, int32_t N, int32_t& max_id_out)
         if (m > max_sc) {
             PerLane<int> is;
             POA_LANES(l) { is[l] = (l < cnt && score[l] == m) ? 1 : 0; }
+            POA_GRAPH_REACH_IF(poa_popc(warp_ballot(is)) > 1, block_max_tie);
             max_id = warp_get(id, poa_ffs(warp_ballot(is)));
             max_sc = m;
+        } else {
+            POA_GRAPH_REACH_IF(m == max_sc, max_tie_across);
         }
     }
     max_id_out = max_id;
 }
+
+#if POA_GRAPH_DIGEST
+POA_FN_NOINLINE unsigned long long cons_digest(const Slot& s_ref, int32_t N, int32_t max_id);
+#endif
 
 POA_FN_NOINLINE void generate_consensus(const Slot& s_ref, const Params p_ref, WinState& st, const WindowOut& out_ref) {
     const Slot s = s_ref;     /* local copies: no reloads of the descriptor after every store */
@@ -2429,11 +2495,23 @@ POA_FN_NOINLINE void generate_consensus(const Slot& s_ref, const Params p_ref, W
     int32_t n = 0;
     int32_t max_id_full = 0;
     consensus_scores_full(s, N, max_id_full);
+    POA_GRAPH_TWIN(consensus, s, N, max_id_full);
+#if POA_GRAPH_DIGEST
+    int32_t max_id_last = 0, rounds = 0;
+    {
+        const unsigned long long d = cons_digest(s, N, max_id_full);
+        POA_LANE0 { out.cons_digest[0] = d; }
+        POA_SYNC();
+    }
+#endif
     POA_LANE0 {
         int32_t max_id = max_id_full;
         POA_SUB_LAP(13);
         int32_t guard = N + 1;
         while (s.nout[max_id] != 0 && guard-- > 0) { /* graph.cpp:520-530 */
+#if POA_GRAPH_DIGEST
+            ++rounds;
+#endif
             const int32_t node_id = max_id;
             const int32_t rank = s.rank_of[node_id];
             /* invalidate the other sources of every out-neighbour (graph.cpp:547-554) */
@@ -2448,6 +2526,9 @@ POA_FN_NOINLINE void generate_consensus(const Slot& s_ref, const Params p_ref, W
             consensus_scores_from(s, N, rank + 1, true, max_id, ms, false);
         }
         POA_SUB_LAP(14);
+#if POA_GRAPH_DIGEST
+        max_id_last = max_id;
+#endif
         /* backtrack into the stack as scratch (path reversed); emitted forward below */
         int32_t v = max_id;
         while (s.c_pred[v] != -1 && n < N) {
@@ -2458,6 +2539,17 @@ POA_FN_NOINLINE void generate_consensus(const Slot& s_ref, const Params p_ref, W
     }
     POA_SYNC();
     n = warp_bcast0(n);
+#if POA_GRAPH_DIGEST
+    {
+        const unsigned long long d = cons_digest(s, N, warp_bcast0(max_id_last));
+        rounds = warp_bcast0(rounds);
+        POA_LANE0 {
+            out.cons_digest[1] = d;
+            *out.cons_rounds = rounds;
+        }
+        POA_SYNC();
+    }
+#endif
     if (n > p.max_cons) {
         st.status = ST_GENERIC_ERROR;
         return;
@@ -2652,7 +2744,7 @@ POA_HD bool score_range_ok(const Params& p, int32_t n_columns, int32_t len) {
     return lo > NEG + 512 && hi < 32000;
 }
 
-#if POA_FILL_DIGEST || POA_ALN_DIGEST
+#if POA_FILL_DIGEST || POA_ALN_DIGEST || POA_GRAPH_DIGEST
 POA_FN unsigned long long digest_mix64(unsigned long long x) { /* splitmix64's finaliser */
     x ^= x >> 30;
     x *= 0xbf58476d1ce4e5b9ull;
@@ -2719,6 +2811,78 @@ POA_FN_NOINLINE unsigned long long aln_digest(const Slot& s_ref, const Params p,
     return digest_warp_sum(acc);
 }
 #endif
+#if POA_GRAPH_DIGEST
+/* Hash of the graph: the wrapping sum over nodes v of
+ *   mix64(v | letter << 16 | rank << 24 | coverage << 40),
+ *   for the aligned id at list position q:  mix64(v | q << 16 | id << 24 | 1 << 56),
+ *   for the in-edge at list position k:     mix64(mix64(v | k << 16 | source << 32 | 2 << 56) + (uint32)weight).
+ * Node ids, letters, the rank order, coverage, the order of every clique and in-edge list and every weight.  The oracle
+ * hashes spoa's graph the same way (poa_oracle_graph_digests). */
+POA_FN_NOINLINE unsigned long long graph_digest(const Slot& s_ref, int32_t N) {
+    const Slot s = s_ref;
+    N = poa_uniform(N);
+    constexpr unsigned long long K = 0x9e3779b97f4a7c15ull;
+    PerLane<unsigned long long> acc;
+    POA_LANES(l) {
+        acc[l] = 0;
+        for (int32_t v = l; v < N; v += 32) {
+            acc[l] += digest_mix64(((unsigned long long)v | ((unsigned long long)s.code[v] << 16) |
+                                    ((unsigned long long)s.rank_of[v] << 24) | ((unsigned long long)s.cov[v] << 40)) + K);
+            const int32_t na = s.aln_cnt[v];
+            for (int32_t q = 0; q < na; ++q)
+                acc[l] += digest_mix64(((unsigned long long)v | ((unsigned long long)q << 16) |
+                                        ((unsigned long long)s.aln[v * KA + q] << 24) | (1ull << 56)) + K);
+            int32_t k = 0;
+            for (uint16_t e = s.in_head[v]; e != NONE16; e = s.e_next[e], ++k) {
+                const unsigned long long h = digest_mix64(((unsigned long long)v | ((unsigned long long)k << 16) |
+                                                           ((unsigned long long)s.e_src[e] << 32) | (2ull << 56)) + K);
+                acc[l] += digest_mix64(h + (unsigned long long)(uint32_t)s.e_w[e]);
+            }
+        }
+    }
+    return digest_warp_sum(acc);
+}
+/* Hash of a subgraph's member order: the wrapping sum over k < n of mix64(k << 32 | sub_at[k] | 3 << 56). */
+POA_FN_NOINLINE unsigned long long sub_digest(const Slot& s_ref, int32_t n) {
+    const Slot s = s_ref;
+    n = poa_uniform(n);
+    PerLane<unsigned long long> acc;
+    POA_LANES(l) {
+        acc[l] = 0;
+        for (int32_t k = l; k < n; k += 32)
+            acc[l] += digest_mix64(((unsigned long long)s.sub_at[k] | ((unsigned long long)k << 32) | (3ull << 56)) +
+                                   0x9e3779b97f4a7c15ull);
+    }
+    return digest_warp_sum(acc);
+}
+/* Hash of the consensus scores: the wrapping sum over nodes v of mix64(mix64(v | 4 << 56) + ((uint32)c_score[v] |
+ * (uint32)c_pred[v] << 32)), plus mix64(max_id | 5 << 56). */
+POA_FN_NOINLINE unsigned long long cons_digest(const Slot& s_ref, int32_t N, int32_t max_id) {
+    const Slot s = s_ref;
+    N = poa_uniform(N);
+    max_id = poa_uniform(max_id);
+    constexpr unsigned long long K = 0x9e3779b97f4a7c15ull;
+    PerLane<unsigned long long> acc;
+    POA_LANES(l) {
+        acc[l] = l == 0 ? digest_mix64(((unsigned long long)(uint32_t)max_id | (5ull << 56)) + K) : 0ull;
+        for (int32_t v = l; v < N; v += 32)
+            acc[l] += digest_mix64(digest_mix64(((unsigned long long)v | (4ull << 56)) + K) +
+                                   ((unsigned long long)(uint32_t)s.c_score[v] |
+                                    ((unsigned long long)(uint32_t)s.c_pred[v] << 32)));
+    }
+    return digest_warp_sum(acc);
+}
+/* after the backbone (r = 0) or after read r was added and sorted */
+POA_FN void record_graph_digest(const Slot& s, const WinState& st, const WindowView& wv, int32_t r) {
+    const unsigned long long d = graph_digest(s, st.n_nodes);
+    POA_LANE0 {
+        wv.graph_digest[r] = d;
+        wv.graph_nodes[r] = st.n_nodes;
+        wv.graph_edges[r] = st.n_edges;
+    }
+    POA_SYNC();
+}
+#endif
 
 /* ------------------------------------------------------------------------------------------
  * One window, start to finish  (racon::Window::generate_consensus, src/window.cpp:65-116, for
@@ -2741,6 +2905,9 @@ POA_FN int32_t process_window(const Slot& s, const Params& p, const WindowView& 
         init_backbone(s, p, st, wv.bases + wv.seq_off[0], wo >= 0 ? wv.weights + wo : nullptr, wo >= 0 ? 0 : (int32_t)(-1 - wo), len0);
         winstate_uniform(st);
         if (wv.path && st.status == ST_SUCCESS) record_path(s.asg, wv.path + wv.seq_off[0], len0, 1);
+#if POA_GRAPH_DIGEST
+        if (st.status == ST_SUCCESS) record_graph_digest(s, st, wv, 0);
+#endif
     }
     for (int32_t r = 1; r < wv.n_seqs && st.status == ST_SUCCESS; ++r) {
         const uint8_t* read = wv.bases + wv.seq_off[r];
@@ -2765,6 +2932,19 @@ POA_FN int32_t process_window(const Slot& s, const Params& p, const WindowView& 
                 break;
             }
             n_rows = poa_uniform(mark_subgraph(s, p, st, sp_begin, sp_end, reinterpret_cast<uint16_t*>(tbs.cells), TB_SCRATCH_BYTES / 2));
+            POA_GRAPH_REACH_IF(sp_begin == 0, sub_begin0);
+            POA_GRAPH_REACH_IF(sp_end == len0 - 1, sub_end_last);
+            POA_GRAPH_TWIN(subgraph, s, p, st, r, sp_begin, sp_end, n_rows, TB_SCRATCH_BYTES / 2);
+#if POA_GRAPH_DIGEST
+            {
+                const unsigned long long d = sub_digest(s, n_rows);
+                POA_LANE0 {
+                    wv.sub_digest[r] = d;
+                    wv.sub_count[r] = n_rows;
+                }
+                POA_SYNC();
+            }
+#endif
         }
         /* static band: one try.  Adaptive band: the configured width is the first try; a traceback that comes close to
          * a band edge (or loses the path) re-aligns this read with twice the width, up to the full matrix. */
@@ -2832,6 +3012,10 @@ POA_FN int32_t process_window(const Slot& s, const Params& p, const WindowView& 
         winstate_uniform(st);
         POA_FENCE();
         tm.lap(PH_TOPSORT);
+        POA_GRAPH_TWIN(topsort, s, p, st, r);
+#if POA_GRAPH_DIGEST
+        record_graph_digest(s, st, wv, r);
+#endif
     }
     if (st.status == ST_SUCCESS && !p.skip_consensus) {
         generate_consensus(s, p, st, out);

@@ -48,9 +48,202 @@ thread_local int32_t* tb_reach_now = nullptr; /* the window the calling thread w
 #define POA_TB_TWIN(fill, ...) (fill).traceback_twin(__VA_ARGS__)
 #define POA_ALN_DIGEST 1 /* WindowView::aln_digest / aln_count: set for every window below */
 
+/* Graph reach report: per window, how often add_alignment, the sorts, the subgraph and the consensus took each of their
+ * paths (tests/emu_lib.py names the fields, tests/graph_cases.py reads them).  poa_core.cuh counts through
+ * POA_GRAPH_REACH; the twins (GraphTwin below) count the rest. */
+enum GraphReach {
+    GR_new_nodes32 = 0, /* reads that add 32 or more new nodes                                           */
+    GR_new_nodes64,     /* ... 64 or more                                                                 */
+    GR_run_cross32,     /* new unaligned nodes whose run's root walk crosses a 32-position boundary       */
+    GR_join1,           /* a new node joins a clique of 1 node (GR_join1 + k: of k + 1 nodes, up to 7)    */
+    GR_join7 = GR_join1 + 6,
+    GR_clique_mate,     /* read positions resolved to an existing aligned node of the same letter         */
+    GR_edge_bumped,     /* edges whose weight a read added to                                              */
+    GR_edge_created,    /* edges created                                                                   */
+    GR_edge_same_root,  /* ... inside one root of the per-root sort (the root is marked dirty)             */
+    GR_edge_cross_root, /* ... across two roots                                                            */
+    GR_du_all,          /* groups of add_alignment_edges with all POA_ADD_DU walks of lane 0 active        */
+    GR_walk_over32,     /* in-edge walks of more than 32 edges                                             */
+    GR_read_len1,       /* reads of one base (they bump no coverage)                                       */
+    GR_const_weights,   /* reads whose bases all weigh one constant                                        */
+    GR_base_weights,    /* reads with per-base weights                                                     */
+    GR_weight0,         /* reads of constant weight 0, and bases of weight 0                               */
+    GR_dirty_over32,    /* sorts with more than 32 dirty multi-node roots (more than one batch of DFS)      */
+    GR_sub_serial,      /* subgraphs ordered by mark_subgraph_serial because the graph exceeds sroot_cap   */
+    GR_sweep_iter2,     /* chunks of the subgraph sweep that took 2 or more iterations                     */
+    GR_sweep_iter3,     /* ... 3 or more                                                                   */
+    GR_straddle,        /* chunks whose lower edge cuts a clique                                           */
+    GR_straddle8,       /* ... a clique of KA + 1 nodes                                                    */
+    GR_sub_begin0,      /* partial-span reads whose span begins at backbone node 0                         */
+    GR_sub_end_last,    /* ... ends at the last backbone node                                              */
+    GR_tie_in_block,    /* consensus: tied in-edges resolved literally, predecessor in the same 32-rank block */
+    GR_tie_pre_block,   /* ... predecessor before the block                                                */
+    GR_tie_equal_pred,  /* ... equal weight and equal predecessor score: '<=' picks the later edge         */
+    GR_block_max_tie,   /* blocks whose maximum score is held by two or more nodes                         */
+    GR_max_tie_across,  /* blocks whose maximum equals the running maximum of the earlier blocks           */
+    GR_topsort_twins,   /* per-root sorts checked against topsort_serial                                   */
+    GR_sub_twins,       /* warp-sweep subgraphs checked against mark_subgraph_serial                       */
+    GR_cons_twins,      /* consensus_scores_full checked against spoa's literal loop                       */
+    GR_twin_mismatches, /* twin checks that found a difference                                             */
+    GR_FIELDS
+};
+/* the first twin check of a window that found a difference: kind (0 sort, 1 subgraph, 2 consensus), read (processing
+ * position; the consensus: -1), index (rank, member position or node; -1: the count or max_id), the twin's value, the
+ * engine's value */
+constexpr int GR_MISMATCH_INTS = 5;
+thread_local int32_t* graph_reach_now = nullptr; /* the window the calling thread works on, or nullptr */
+#define POA_GRAPH_REACH(field) (graph_reach_now ? (void)(graph_reach_now[GR_##field] += 1) : (void)0)
+#define POA_GRAPH_REACH_IF(cond, field) ((cond) ? POA_GRAPH_REACH(field) : (void)0)
+#define POA_GRAPH_REACH_AT(field, k) (graph_reach_now ? (void)(graph_reach_now[GR_##field + (k)] += 1) : (void)0)
+#define POA_GRAPH_TWIN(what, ...) graph_twin_##what(__VA_ARGS__)
+#define POA_GRAPH_DIGEST 1 /* WindowView::graph_digest ..., WindowOut::cons_digest / cons_rounds: set below */
+namespace b200poa {
+struct Slot;
+struct Params;
+struct WinState;
+}
+static void graph_twin_topsort(const b200poa::Slot& s, const b200poa::Params& p, const b200poa::WinState& st, int32_t r);
+static void graph_twin_subgraph(const b200poa::Slot& s, const b200poa::Params& p, const b200poa::WinState& st,
+                                int32_t r, int32_t begin, int32_t end, int32_t n, int32_t cap);
+static void graph_twin_consensus(const b200poa::Slot& s, int32_t N, int32_t max_id);
+static void graph_twin_sweep_chunk(const b200poa::Slot& s, int32_t hi);
+static void graph_twin_sweep_step();
+
 #include "../../racon_gpu_b200/csrc/poa_core.cuh"
 
 using namespace b200poa;
+
+/* Twins of the graph phases.  Each runs on shadow copies of the arrays it writes (the graph itself is only read), so
+ * that it cannot change what the engine does next. */
+struct GraphTwin {
+    int32_t* reach = nullptr;    /* this window's report (GR_FIELDS) */
+    int32_t* mismatch = nullptr; /* this window's first mismatch (GR_MISMATCH_INTS), or nullptr */
+    int32_t sweep_steps = 0;
+    std::vector<uint8_t> marks, check;
+    std::vector<uint16_t> stack, node_at, rank_of, sub_at, sub_rank;
+    std::vector<uint32_t> row_meta, roff;
+    std::vector<int32_t> c_score, c_pred;
+
+    void size(const Params& p) {
+        const size_t MN = (size_t)p.max_nodes, ME = (size_t)p.max_edges;
+        marks.resize(MN);
+        check.resize(MN);
+        stack.resize(ME + (KA + 2) * MN);
+        node_at.resize(MN);
+        rank_of.resize(MN);
+        sub_at.resize(MN);
+        sub_rank.resize(MN);
+        row_meta.resize(MN);
+        roff.resize(MN + 1);
+        c_score.resize(MN);
+        c_pred.resize(MN);
+    }
+    Slot shadow(const Slot& s) {
+        Slot t = s;
+        t.marks = marks.data();
+        t.check = check.data();
+        t.stack = stack.data();
+        t.node_at = node_at.data();
+        t.rank_of = rank_of.data();
+        t.sub_at = sub_at.data();
+        t.sub_rank = sub_rank.data();
+        t.row_meta = row_meta.data();
+        t.roff = roff.data();
+        t.c_score = c_score.data();
+        t.c_pred = c_pred.data();
+        return t;
+    }
+    void report(int32_t kind, int32_t r, int32_t idx, int32_t twin, int32_t eng) {
+        reach[GR_twin_mismatches] += 1;
+        if (mismatch && mismatch[0] < 0) {
+            const int32_t m[GR_MISMATCH_INTS] = {kind, r, idx, twin, eng};
+            std::copy(m, m + GR_MISMATCH_INTS, mismatch);
+        }
+    }
+};
+thread_local GraphTwin* graph_twin_now = nullptr;
+
+/* after every per-root sort: topsort_serial must give the same rank order */
+static void graph_twin_topsort(const Slot& s, const Params& p, const WinState& st, int32_t r) {
+    GraphTwin* g = graph_twin_now;
+    if (!g || p.serial_topsort) return;
+    g->reach[GR_topsort_twins] += 1;
+    const Slot t = g->shadow(s);
+    WinState ts = st;
+    topsort_serial(t, p, ts);
+    for (int32_t k = 0; k < st.n_nodes; ++k)
+        if (t.node_at[k] != s.node_at[k]) {
+            g->report(0, r, k, t.node_at[k], s.node_at[k]);
+            return;
+        }
+}
+
+/* after every warp-sweep subgraph: mark_subgraph_serial must give the same members in the same order */
+static void graph_twin_subgraph(const Slot& s, const Params& p, const WinState& st, int32_t r, int32_t begin,
+                                int32_t end, int32_t n, int32_t cap) {
+    GraphTwin* g = graph_twin_now;
+    if (!g || p.serial_topsort || st.n_nodes > cap) return; /* the engine ran the serial order itself */
+    g->reach[GR_sub_twins] += 1;
+    const Slot t = g->shadow(s);
+    WinState ts = st;
+    const int32_t tn = mark_subgraph_serial(t, p, ts, begin, end);
+    if (tn != n) {
+        g->report(1, r, -1, tn, n);
+        return;
+    }
+    for (int32_t k = 0; k < n; ++k)
+        if (t.sub_at[k] != s.sub_at[k]) {
+            g->report(1, r, k, t.sub_at[k], s.sub_at[k]);
+            return;
+        }
+}
+
+/* after consensus_scores_full: spoa's literal loop (graph.cpp:494-518, scores and predecessors -1 everywhere to start,
+ * "scores[max_score_id] < scores[id]") must give the same scores, predecessors and max_id */
+static void graph_twin_consensus(const Slot& s, int32_t N, int32_t max_id) {
+    GraphTwin* g = graph_twin_now;
+    if (!g) return;
+    g->reach[GR_cons_twins] += 1;
+    const Slot t = g->shadow(s);
+    std::fill(g->c_score.begin(), g->c_score.begin() + N, -1);
+    std::fill(g->c_pred.begin(), g->c_pred.begin() + N, -1);
+    for (int32_t k = 0; k < N; ++k) t.node_at[k] = s.node_at[k];
+    int32_t tmax = 0, unused = 0;
+    consensus_scores_from(t, N, 0, false, tmax, unused, true);
+    for (int32_t v = 0; v < N; ++v) {
+        if (t.c_score[v] != s.c_score[v]) {
+            g->report(2, -1, v, t.c_score[v], s.c_score[v]);
+            return;
+        }
+        if (t.c_pred[v] != s.c_pred[v]) {
+            g->report(2, -1, v, t.c_pred[v], s.c_pred[v]);
+            return;
+        }
+    }
+    if (tmax != max_id) g->report(2, -1, -1, tmax, max_id);
+}
+
+/* the subgraph sweep: a chunk [hi - 31, hi] begins (does its lower edge cut a clique?), one iteration of a chunk ran */
+static void graph_twin_sweep_chunk(const Slot& s, int32_t hi) {
+    GraphTwin* g = graph_twin_now;
+    if (!g) return;
+    g->sweep_steps = 0;
+    const int32_t lo = hi - 31;
+    if (lo < 1) return;
+    const int32_t a = s.node_at[lo], b = s.node_at[lo - 1];
+    for (int32_t q = 0; q < s.aln_cnt[a]; ++q)
+        if (s.aln[a * KA + q] == b) {
+            g->reach[GR_straddle] += 1;
+            if (s.aln_cnt[a] == KA) g->reach[GR_straddle8] += 1;
+        }
+}
+static void graph_twin_sweep_step() {
+    GraphTwin* g = graph_twin_now;
+    if (!g) return;
+    ++g->sweep_steps;
+    if (g->sweep_steps == 2) g->reach[GR_sweep_iter2] += 1;
+    if (g->sweep_steps == 3) g->reach[GR_sweep_iter3] += 1;
+}
 
 namespace {
 
@@ -258,9 +451,9 @@ extern "C" {
 
 /* Flat batch in ADD order + order[] (processing permutation), like poa_oracle_polish_windows.
  * Outputs the UNTRIMMED consensus, coverage and the per-window status.  rank_out (nullable):
- * n_windows x max_nodes final rank_to_node order, n_nodes_out (nullable) node counts.  emu_polish_windows (below) is
- * the same without the traceback's outputs. */
-void emu_polish_windows_tb(int64_t n_windows, const int64_t* win_seq_off, const int64_t* seq_off,
+ * n_windows x max_nodes final rank_to_node order, n_nodes_out (nullable) node counts.  emu_polish_windows_tb and
+ * emu_polish_windows (below) are the same without the graph's, and without the traceback's, outputs. */
+void emu_polish_windows_graph(int64_t n_windows, const int64_t* win_seq_off, const int64_t* seq_off,
                         const uint8_t* bases, const int8_t* weights, const uint8_t* has_weights,
                         const int32_t* begins, const int32_t* ends, const int32_t* order, int32_t m, int32_t x, int32_t gap,
                         int32_t max_nodes, int32_t max_edges, int32_t max_len, int32_t band_width,
@@ -277,7 +470,15 @@ void emu_polish_windows_tb(int64_t n_windows, const int64_t* win_seq_off, const 
                          * count.  Per window (nullable): TB_FIELDS traceback reach counters, and the first traceback
                          * that differs from the scalar twin (TB_MISMATCH_INTS, read -1: none). */
                         unsigned long long* aln_digest_out, int32_t* aln_count_out, int32_t* tb_reach_out,
-                        int32_t* tb_mismatch_out) {
+                        int32_t* tb_mismatch_out,
+                        /* Per sequence (nullable): graph_digest() after it was added and sorted, the graph's node and
+                         * edge counts, and for partial-span reads sub_digest() and the member count.  Per window
+                         * (nullable): cons_digest() after the full scoring pass and after branch completion, the rounds
+                         * of branch completion, GR_FIELDS graph reach counters and the first twin check that found a
+                         * difference (GR_MISMATCH_INTS, kind -1: none). */
+                        unsigned long long* graph_digest_out, int32_t* graph_nodes_out, int32_t* graph_edges_out,
+                        unsigned long long* sub_digest_out, int32_t* sub_count_out, unsigned long long* cons_digest_out,
+                        int32_t* cons_rounds_out, int32_t* graph_reach_out, int32_t* graph_mismatch_out) {
     Params p;
     p.max_nodes = max_nodes;
     p.max_edges = poa_edge_capacity(max_nodes); /* the engine derives the edge pool from the node capacity */
@@ -319,6 +520,9 @@ void emu_polish_windows_tb(int64_t n_windows, const int64_t* win_seq_off, const 
         std::vector<uint8_t> tb_mem(TB_SCRATCH_BYTES + 64);
         TbScratch tbs;
         tb_bind(tbs, reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(tb_mem.data()) + 15) & ~uintptr_t(15)));
+        GraphTwin twin;
+        twin.size(p);
+        std::vector<int32_t> gr_scratch(GR_FIELDS);
         for (;;) {
             const int64_t w = cursor.fetch_add(1);
             if (w >= n_windows) break;
@@ -395,6 +599,22 @@ void emu_polish_windows_tb(int64_t n_windows, const int64_t* win_seq_off, const 
             if (fill.tb_mismatch)
                 for (int32_t k = 0; k < TB_MISMATCH_INTS; ++k) fill.tb_mismatch[k] = -1;
             fill.tb_last_read = nullptr;
+            std::vector<unsigned long long> wgraph((size_t)n, 0), wsub((size_t)n, 0);
+            std::vector<int32_t> wnodes((size_t)n, 0), wedges((size_t)n, 0), wsubcnt((size_t)n, 0);
+            wv.graph_digest = wgraph.data();
+            wv.graph_nodes = wnodes.data();
+            wv.graph_edges = wedges.data();
+            wv.sub_digest = wsub.data();
+            wv.sub_count = wsubcnt.data();
+            unsigned long long wcons[2] = {0, 0};
+            int32_t wrounds = 0;
+            twin.reach = graph_reach_out ? graph_reach_out + w * GR_FIELDS : gr_scratch.data();
+            for (int32_t k = 0; k < GR_FIELDS; ++k) twin.reach[k] = 0;
+            twin.mismatch = graph_mismatch_out ? graph_mismatch_out + w * GR_MISMATCH_INTS : nullptr;
+            if (twin.mismatch)
+                for (int32_t k = 0; k < GR_MISMATCH_INTS; ++k) twin.mismatch[k] = -1;
+            graph_reach_now = twin.reach;
+            graph_twin_now = &twin;
             /* process_window writes its node count nowhere; recover it from the slot afterwards */
             uint32_t cursor = 0;
             int32_t off = 0, trim = 0;
@@ -407,10 +627,26 @@ void emu_polish_windows_tb(int64_t n_windows, const int64_t* win_seq_off, const 
             out.off = &off;
             out.trim = &trim;
             out.trim_nseq = n;
+            out.cons_digest = wcons;
+            out.cons_rounds = &wrounds;
             long long moff = 0;
             int32_t mcols = 0, mst = 0;
             const int32_t n_final = process_window(s, p, wv, fill, tbs, out);
             tb_reach_now = nullptr;
+            graph_reach_now = nullptr;
+            graph_twin_now = nullptr;
+            for (int32_t k = 0; k < n; ++k) {
+                if (graph_digest_out) graph_digest_out[s0 + k] = wgraph[(size_t)k];
+                if (graph_nodes_out) graph_nodes_out[s0 + k] = wnodes[(size_t)k];
+                if (graph_edges_out) graph_edges_out[s0 + k] = wedges[(size_t)k];
+                if (sub_digest_out) sub_digest_out[s0 + k] = wsub[(size_t)k];
+                if (sub_count_out) sub_count_out[s0 + k] = wsubcnt[(size_t)k];
+            }
+            if (cons_digest_out) {
+                cons_digest_out[2 * w] = wcons[0];
+                cons_digest_out[2 * w + 1] = wcons[1];
+            }
+            if (cons_rounds_out) cons_rounds_out[w] = wrounds;
             if (aln_digest_out)
                 for (int32_t k = 0; k < n; ++k) aln_digest_out[s0 + k] = waln[(size_t)k];
             if (aln_count_out)
@@ -463,6 +699,25 @@ void emu_polish_windows_tb(int64_t n_windows, const int64_t* win_seq_off, const 
     if (cells_out) *cells_out = total_cells.load();
     (void)rank_out;
     (void)n_nodes_out;
+}
+
+void emu_polish_windows_tb(int64_t n_windows, const int64_t* win_seq_off, const int64_t* seq_off,
+                           const uint8_t* bases, const int8_t* weights, const uint8_t* has_weights,
+                           const int32_t* begins, const int32_t* ends, const int32_t* order, int32_t m, int32_t x,
+                           int32_t gap, int32_t max_nodes, int32_t max_edges, int32_t max_len, int32_t band_width,
+                           int32_t serial_topsort, int32_t n_threads, uint8_t* cons_out, uint16_t* cov_out,
+                           int32_t stride_out, int32_t* cons_len, int32_t* status, int32_t* rank_out,
+                           int32_t* n_nodes_out, int64_t* cells_out, int32_t* trim_out, uint8_t* msa_out,
+                           int64_t msa_cap, int64_t* msa_off, int32_t* msa_cols, int32_t* msa_status, int32_t ring_rows,
+                           unsigned long long* digest_out, int32_t* fill_count_out, int32_t* reach_out,
+                           unsigned long long* aln_digest_out, int32_t* aln_count_out, int32_t* tb_reach_out,
+                           int32_t* tb_mismatch_out) {
+    emu_polish_windows_graph(n_windows, win_seq_off, seq_off, bases, weights, has_weights, begins, ends, order, m, x,
+                             gap, max_nodes, max_edges, max_len, band_width, serial_topsort, n_threads, cons_out,
+                             cov_out, stride_out, cons_len, status, rank_out, n_nodes_out, cells_out, trim_out, msa_out,
+                             msa_cap, msa_off, msa_cols, msa_status, ring_rows, digest_out, fill_count_out, reach_out,
+                             aln_digest_out, aln_count_out, tb_reach_out, tb_mismatch_out, nullptr, nullptr, nullptr,
+                             nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
 }
 
 void emu_polish_windows(int64_t n_windows, const int64_t* win_seq_off, const int64_t* seq_off,

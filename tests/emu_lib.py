@@ -21,6 +21,15 @@ TB_REACH_FIELDS = ("tracebacks", "tile_loads", "reanchors", "global_npred", "glo
                    "count_mod0", "count_mod1", "count_mod31", "i32_reads", "partial_reads", "twin_mismatches")
 #: the first traceback of a window that differs from the scalar twin (read -1: none), in order
 TB_MISMATCH_FIELDS = ("read", "try", "entry", "twin_node", "twin_pos", "node", "pos", "twin_count", "count")
+#: per-window reach counters of the emulated graph phases (enum GraphReach in tests/emu/emu_poa.cpp), in order
+GRAPH_REACH_FIELDS = ("new_nodes32", "new_nodes64", "run_cross32", "join1", "join2", "join3", "join4", "join5", "join6",
+                      "join7", "clique_mate", "edge_bumped", "edge_created", "edge_same_root", "edge_cross_root",
+                      "du_all", "walk_over32", "read_len1", "const_weights", "base_weights", "weight0", "dirty_over32",
+                      "sub_serial", "sweep_iter2", "sweep_iter3", "straddle", "straddle8", "sub_begin0",
+                      "sub_end_last", "tie_in_block", "tie_pre_block", "tie_equal_pred", "block_max_tie",
+                      "max_tie_across", "topsort_twins", "sub_twins", "cons_twins", "twin_mismatches")
+#: the first graph twin check of a window that found a difference (kind -1: none; 0 sort, 1 subgraph, 2 consensus)
+GRAPH_MISMATCH_FIELDS = ("kind", "read", "index", "twin", "engine")
 
 
 class Emu:
@@ -37,7 +46,10 @@ class Emu:
         ring_rows: the GPU launch's score-row ring, which decides the row program's far-predecessor flags.
         Also per sequence the digest and entry count of the alignment added to the graph (last_aln_digest,
         last_aln_count), per window the traceback's reach counters (last_tb_reach: dict TB_REACH_FIELDS -> array) and
-        its first difference from the scalar twin walk (last_tb_mismatch: W x TB_MISMATCH_FIELDS, read -1: none)."""
+        its first difference from the scalar twin walk (last_tb_mismatch: W x TB_MISMATCH_FIELDS, read -1: none).
+        And the graph phases' outputs (last_graph: dict of per-sequence graph_digest, graph_nodes, graph_edges,
+        sub_digest, sub_count, per-window cons_digest (W x 2) and cons_rounds), their reach counters (last_graph_reach:
+        dict GRAPH_REACH_FIELDS -> array) and first twin difference (last_graph_mismatch: W x GRAPH_MISMATCH_FIELDS)."""
         W = b.n_windows
         cons = np.zeros((W, stride), dtype=np.uint8)
         cov = np.zeros((W, stride), dtype=np.uint16)
@@ -52,9 +64,16 @@ class Emu:
         self.last_aln_count = np.zeros(b.n_seqs, dtype=np.int32)
         tb_reach = np.zeros((W, len(TB_REACH_FIELDS)), dtype=np.int32)
         self.last_tb_mismatch = np.full((W, len(TB_MISMATCH_FIELDS)), -1, dtype=np.int32)
+        n = b.n_seqs
+        gr = {"graph_digest": np.zeros(n, dtype=np.uint64), "graph_nodes": np.zeros(n, dtype=np.int32),
+              "graph_edges": np.zeros(n, dtype=np.int32), "sub_digest": np.zeros(n, dtype=np.uint64),
+              "sub_count": np.zeros(n, dtype=np.int32), "cons_digest": np.zeros((W, 2), dtype=np.uint64),
+              "cons_rounds": np.zeros(W, dtype=np.int32)}
+        g_reach = np.zeros((W, len(GRAPH_REACH_FIELDS)), dtype=np.int32)
+        self.last_graph_mismatch = np.full((W, len(GRAPH_MISMATCH_FIELDS)), -1, dtype=np.int32)
         order = np.ascontiguousarray(order, dtype=np.int32)
         a = _flat_args(b)
-        self.lib.emu_polish_windows_tb(
+        self.lib.emu_polish_windows_graph(
             a[0], a[1], a[2], a[3], a[4], a[5], a[6], a[7], _p(order, C.c_int32), C.c_int32(m), C.c_int32(x), C.c_int32(g),
             C.c_int32(max_nodes), C.c_int32(max_edges), C.c_int32(max_len), C.c_int32(band),
             C.c_int32(int(serial_topsort)), C.c_int32(threads), _p(cons, C.c_uint8), _p(cov, C.c_uint16),
@@ -62,7 +81,12 @@ class Emu:
             _p(self.last_trim, C.c_int32), *self._msa_args(W, msa_cap), C.c_int32(ring_rows),
             _p(self.last_digest, C.c_uint64), _p(self.last_fill_count, C.c_int32), _p(reach, C.c_int32),
             _p(self.last_aln_digest, C.c_uint64), _p(self.last_aln_count, C.c_int32), _p(tb_reach, C.c_int32),
-            _p(self.last_tb_mismatch, C.c_int32))
+            _p(self.last_tb_mismatch, C.c_int32), _p(gr["graph_digest"], C.c_uint64), _p(gr["graph_nodes"], C.c_int32),
+            _p(gr["graph_edges"], C.c_int32), _p(gr["sub_digest"], C.c_uint64), _p(gr["sub_count"], C.c_int32),
+            _p(gr["cons_digest"], C.c_uint64), _p(gr["cons_rounds"], C.c_int32), _p(g_reach, C.c_int32),
+            _p(self.last_graph_mismatch, C.c_int32))
+        self.last_graph = gr
+        self.last_graph_reach = {k: g_reach[:, i].copy() for i, k in enumerate(GRAPH_REACH_FIELDS)}
         self.last_reach = {k: reach[:, i].copy() for i, k in enumerate(REACH_FIELDS)}
         self.last_tb_reach = {k: tb_reach[:, i].copy() for i, k in enumerate(TB_REACH_FIELDS)}
         self.last_msa = None

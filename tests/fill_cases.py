@@ -277,7 +277,9 @@ def emu_run(emu, r, ring_rows: int, msa: bool = True):
     return {"status": st, "cons": cons, "cov": cov, "msa": emu.last_msa, "digest": emu.last_digest.copy(),
             "count": emu.last_fill_count.copy(), "reach": emu.last_reach, "aln_digest": emu.last_aln_digest.copy(),
             "aln_count": emu.last_aln_count.copy(), "tb_reach": emu.last_tb_reach,
-            "tb_mismatch": emu.last_tb_mismatch.copy()}
+            "tb_mismatch": emu.last_tb_mismatch.copy(), "trim": emu.last_trim.copy(),
+            "graph": {k: v.copy() for k, v in emu.last_graph.items()}, "graph_reach": emu.last_graph_reach,
+            "graph_mismatch": emu.last_graph_mismatch.copy()}
 
 
 def ring_rows_of(r) -> int:
@@ -430,6 +432,18 @@ def _gpu_job(r):
                                               acnt.ctypes.data_as(C.POINTER(C.c_int32)), C.c_int64(b.n_seqs))
             assert st == api.SUCCESS, api.status_string(st)
             out.update(aln_digest=adg, aln_count=acnt)
+            n, W = b.n_seqs, b.n_windows
+            gr = {"graph_digest": np.zeros(n, dtype=np.uint64), "graph_nodes": np.zeros(n, dtype=np.int32),
+                  "graph_edges": np.zeros(n, dtype=np.int32), "sub_digest": np.zeros(n, dtype=np.uint64),
+                  "sub_count": np.zeros(n, dtype=np.int32), "cons_digest": np.zeros((W, 2), dtype=np.uint64),
+                  "cons_rounds": np.zeros(W, dtype=np.int32)}
+            ptr = {k: v.ctypes.data_as(C.POINTER(C.c_uint64 if v.dtype == np.uint64 else C.c_int32))
+                   for k, v in gr.items()}
+            st = lib.b200poa_debug_graph_digest(pb.handle, ptr["graph_digest"], ptr["graph_nodes"], ptr["graph_edges"],
+                                                ptr["sub_digest"], ptr["sub_count"], C.c_int64(n), ptr["cons_digest"],
+                                                ptr["cons_rounds"], C.c_int64(W))
+            assert st == api.SUCCESS, api.status_string(st)
+            out.update(graph=gr)
         pb.close()
         return out
     finally:
@@ -455,14 +469,42 @@ def aln_digest_failures(name, b, got, want, what="emulation") -> list:
     return bad
 
 
+SEQ_FIELDS = ("graph_digest", "graph_nodes", "graph_edges", "sub_digest", "sub_count")
+
+
+def graph_digest_failures(name, b, got, want, what="emulation", windows=None) -> list:
+    """Per window (all, or those listed), the first read (processing position) whose graph or subgraph digest or count
+    differs, and a differing consensus digest or round count."""
+    bad = []
+    for w in (range(b.n_windows) if windows is None else windows):
+        s0, s1 = int(b.win_seq_off[w]), int(b.win_seq_off[w + 1])
+        for k in range(s1 - s0):
+            diff = [f for f in SEQ_FIELDS if got[f][s0 + k] != want[f][s0 + k]]
+            if diff:
+                bad.append(f"{name}: window {w} read {k}: {', '.join(diff)} differ from the {what} ("
+                           f"{got['graph_nodes'][s0 + k]} nodes {got['graph_edges'][s0 + k]} edges, {what} "
+                           f"{want['graph_nodes'][s0 + k]} nodes {want['graph_edges'][s0 + k]} edges)")
+                break
+        for j, when in enumerate(("after the scoring pass", "after branch completion")):
+            if got["cons_digest"][w][j] != want["cons_digest"][w][j]:
+                bad.append(f"{name}: window {w}: consensus scores {when} differ from the {what}")
+        if got["cons_rounds"][w] != want["cons_rounds"][w]:
+            bad.append(f"{name}: window {w}: {got['cons_rounds'][w]} rounds of branch completion, {what} "
+                       f"{want['cons_rounds'][w]}")
+    return bad
+
+
+
 def compare(r, got, want, oracle_out=None) -> list:
     """Differences between a GPU run and the emulation (and, in full band, the oracle).  Digest mismatches name the
     window, the read (processing position) and how many fills it took; alignment digests (where both sides have them)
-    the read and its entry counts."""
+    the read and its entry counts; graph digests the read and its node and edge counts."""
     b = r["batch"]
     bad = []
     if "aln_digest" in got and "aln_digest" in want:
         bad += aln_digest_failures(r["name"], b, got, want)
+    if "graph" in got and "graph" in want:
+        bad += graph_digest_failures(r["name"], b, got["graph"], want["graph"])
     if "digest" in got:
         for w in range(b.n_windows):
             s0, s1 = int(b.win_seq_off[w]), int(b.win_seq_off[w + 1])

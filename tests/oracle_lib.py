@@ -75,6 +75,26 @@ class Oracle:
                                               _p(cnt, C.c_int32))
         return dg, cnt
 
+    def graph_digests(self, batch, order: np.ndarray, m: int, x: int, g: int, threads: int = 16) -> dict:
+        """spoa's graphs hashed the way the engine's test build hashes its own (poa_oracle_graph_digests): per sequence
+        (ADD-order index of the window's first sequence + processing position) graph_digest, graph_nodes, graph_edges,
+        sub_digest and sub_count; per window cons_digest (W x 2), cons_rounds, overflow (weights or scores that do
+        not fit 32 bits) and max_indegree (the largest in-degree of the final graph)."""
+        n, W = batch.n_seqs, batch.n_windows
+        out = {"graph_digest": np.zeros(n, dtype=np.uint64), "graph_nodes": np.zeros(n, dtype=np.int32),
+               "graph_edges": np.zeros(n, dtype=np.int32), "sub_digest": np.zeros(n, dtype=np.uint64),
+               "sub_count": np.zeros(n, dtype=np.int32), "cons_digest": np.zeros((W, 2), dtype=np.uint64),
+               "cons_rounds": np.zeros(W, dtype=np.int32), "overflow": np.zeros(W, dtype=np.int64),
+               "max_indegree": np.zeros(W, dtype=np.int32)}
+        order = np.ascontiguousarray(order, dtype=np.int32)
+        self.lib.poa_oracle_graph_digests.restype = None
+        self.lib.poa_oracle_graph_digests(
+            *_flat_args(batch), _p(order, C.c_int32), C.c_int32(m), C.c_int32(x), C.c_int32(g), C.c_int32(threads),
+            _p(out["graph_digest"], C.c_uint64), _p(out["graph_nodes"], C.c_int32), _p(out["graph_edges"], C.c_int32),
+            _p(out["sub_digest"], C.c_uint64), _p(out["sub_count"], C.c_int32), _p(out["cons_digest"], C.c_uint64),
+            _p(out["cons_rounds"], C.c_int32), _p(out["overflow"], C.c_int64), _p(out["max_indegree"], C.c_int32))
+        return out
+
 
 def _seq_arrays(seqs, weights):
     n = len(seqs)
