@@ -38,6 +38,15 @@ SPLIT_REC_DTYPE = np.dtype([("aln", "<i4"), ("r0", "<i4"), ("c0", "<i4"), ("n", 
 SPLIT_PATHS = ("warp", "team", "side")  # one warp; a team in a thin level; a team on the side stream
 SPLIT_TIMEOUT = 1
 
+#: one record of the test build's leaf log (aln_core.cuh AlnLeafRec, b200aln_debug_leaf_log): a leaf -- the sub-problem,
+#: the band its pass got, its flags (bit 0 top level, bit 1 guessed band), the score at its last cell, the walk's counters
+#: (LEAF_COUNTERS), the cells its pass computed and an order-independent hash of its (n + m)-byte operations region
+LEAF_COUNTERS = ("diag_rounds", "diag_ops", "matches", "up_rounds", "left_rounds", "full_runs", "reload_block",
+                 "reload_col", "border_lanes", "tail", "tail_kind")
+LEAF_REC_DTYPE = np.dtype([("aln", "<i4"), ("r0", "<i4"), ("c0", "<i4"), ("n", "<i4"), ("m", "<i4"), ("band", "<i4"),
+                           ("top", "<i4"), ("score", "<i4")] + [(k, "<i4") for k in LEAF_COUNTERS]
+                          + [("pad", "<i4"), ("cells", "<i8"), ("ops_hash", "<u8")])
+
 
 def is_leaf(n: int, m: int) -> bool:
     """aln_core.cuh aln_is_leaf (edlib.cpp:1135-1157): is an n x m sub-problem traced back without a split?"""
@@ -216,20 +225,28 @@ class CUDABatchAligner:
     def split_log(self) -> np.ndarray:
         """Test build only (racon_gpu_b200/variants/libb200poa_digest.so): the split log of the last align_all, one
         SPLIT_REC_DTYPE record per split attempt.  Raises when the log overflowed."""
-        fn = getattr(self.lib, "b200aln_debug_split_log", None)
+        return self._debug_log("b200aln_debug_split_log", SPLIT_REC_DTYPE, "split")
+
+    def leaf_log(self) -> np.ndarray:
+        """Test build only: the leaf log of the last align_all, one LEAF_REC_DTYPE record per leaf.  Raises when the log
+        overflowed."""
+        return self._debug_log("b200aln_debug_leaf_log", LEAF_REC_DTYPE, "leaf")
+
+    def _debug_log(self, name, dtype, what) -> np.ndarray:
+        fn = getattr(self.lib, name, None)
         if fn is None:
-            raise RuntimeError("this library has no split log: load the digest build")
+            raise RuntimeError(f"this library has no {what} log: load the digest build")
         count, rec_bytes = C.c_int64(0), C.c_int32(0)
         st = fn(self.h, None, C.c_int64(0), C.byref(count), C.byref(rec_bytes))
         if st not in (SUCCESS, GENERIC_ERROR):
-            raise RuntimeError(f"b200aln_debug_split_log: {status_string(st)}")
-        assert rec_bytes.value == SPLIT_REC_DTYPE.itemsize, (rec_bytes.value, SPLIT_REC_DTYPE.itemsize)
-        out = np.zeros(count.value, dtype=SPLIT_REC_DTYPE)
+            raise RuntimeError(f"{name}: {status_string(st)}")
+        assert rec_bytes.value == dtype.itemsize, (rec_bytes.value, dtype.itemsize)
+        out = np.zeros(count.value, dtype=dtype)
         st = fn(self.h, out.ctypes.data_as(C.c_void_p), C.c_int64(count.value), C.byref(count), C.byref(rec_bytes))
         if st == GENERIC_ERROR:
-            raise RuntimeError(f"the split log overflowed: {count.value} records appended")
+            raise RuntimeError(f"the {what} log overflowed: {count.value} records appended")
         if st != SUCCESS:
-            raise RuntimeError(f"b200aln_debug_split_log: {status_string(st)}")
+            raise RuntimeError(f"{name}: {status_string(st)}")
         return out
 
 

@@ -36,9 +36,12 @@ def _nvcc() -> str:
 #: with hashes of its middle columns (aln_core.cuh ALN_SPLIT_DIGEST, b200aln_debug_split_log), and every alignment the
 #: POA traceback adds to a graph hashed per sequence (poa_core.cuh POA_ALN_DIGEST, b200poa_debug_aln_digest), and the
 #: graph after every read, every subgraph and the consensus scores hashed (poa_core.cuh POA_GRAPH_DIGEST,
-#: b200poa_debug_graph_digest).  Same sources and flags as the product plus these defines.
+#: b200poa_debug_graph_digest), and every leaf of the overlap aligner logged with its end score, a hash of its operations
+#: and the walk's counters (aln_core.cuh ALN_LEAF_DIGEST, b200aln_debug_leaf_log).  Same sources and flags as the
+#: product plus these defines.
 DIGEST_LIB = os.path.join(HERE, "variants", "libb200poa_digest.so")
-DIGEST_FLAGS = ["-DPOA_FILL_DIGEST=1", "-DALN_SPLIT_DIGEST=1", "-DPOA_ALN_DIGEST=1", "-DPOA_GRAPH_DIGEST=1"]
+DIGEST_FLAGS = ["-DPOA_FILL_DIGEST=1", "-DALN_SPLIT_DIGEST=1", "-DPOA_ALN_DIGEST=1", "-DPOA_GRAPH_DIGEST=1",
+                "-DALN_LEAF_DIGEST=1"]
 
 
 def needs_build(lib: str = LIB) -> bool:

@@ -264,6 +264,9 @@ POA_FN int64_t leaf_entry(int32_t b, int32_t j, int32_t B, int32_t cols) {
 #ifndef ALN_SPLIT_DIGEST
 #define ALN_SPLIT_DIGEST 0
 #endif
+#ifndef ALN_LEAF_DIGEST
+#define ALN_LEAF_DIGEST 0
+#endif
 #if ALN_EMU_TEAMS && POA_DEVICE
 #error "ALN_EMU_TEAMS is the host emulation's"
 #endif
@@ -716,7 +719,7 @@ POA_FN_NOINLINE int64_t aln_split(const AlnSlot& s_ref, EqTab& eq, const uint8_t
     return cells;
 }
 
-#if ALN_SPLIT_DIGEST || !POA_DEVICE
+#if ALN_SPLIT_DIGEST || ALN_LEAF_DIGEST || !POA_DEVICE
 /* Test builds: one record per split attempt (b200aln_debug_split_log on the device, the batch emulation in tests/emu),
  * so that every Hirschberg step -- both middle columns, the split -- can be compared between the two. */
 enum { ALN_PATH_WARP = 0, ALN_PATH_TEAM = 1, ALN_PATH_SIDE = 2 }; /* one warp; a team in a thin level; a team on the side stream */
@@ -738,6 +741,18 @@ POA_FN unsigned long long aln_mix64(unsigned long long x) { /* splitmix64's fina
     x ^= x >> 31;
     return x;
 }
+POA_FN unsigned long long aln_warp_sum64(const PerLane<unsigned long long>& acc) { /* wrapping; every lane gets it */
+#if POA_DEVICE
+    unsigned long long t = acc[0];
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) t += __shfl_xor_sync(0xffffffffu, t, d);
+    return t;
+#else
+    unsigned long long t = 0;
+    for (int l = 0; l < 32; ++l) t += acc[l];
+    return t;
+#endif
+}
 /* Hash of a middle column: the wrapping sum over rows i = 0..n of mix64(i, col[i]), independent of the order lanes visit
  * the rows in.  Whole warp. */
 POA_FN_NOINLINE unsigned long long aln_col_digest(const int32_t* col, int32_t n) {
@@ -750,17 +765,55 @@ POA_FN_NOINLINE unsigned long long aln_col_digest(const int32_t* col, int32_t n)
             if (i <= n) acc[l] += aln_mix64((((unsigned long long)(uint32_t)i << 32) | (uint32_t)col[i]) + 0x9e3779b97f4a7c15ull);
         }
     }
-#if POA_DEVICE
-    unsigned long long t = acc[0];
-#pragma unroll
-    for (int d = 16; d > 0; d >>= 1) t += __shfl_xor_sync(0xffffffffu, t, d);
-    return t;
-#else
-    unsigned long long t = 0;
-    for (int l = 0; l < 32; ++l) t += acc[l];
-    return t;
-#endif
+    return aln_warp_sum64(acc);
 }
+#endif
+
+#if ALN_LEAF_DIGEST || !POA_DEVICE
+/* Test builds: one record per leaf (b200aln_debug_leaf_log on the device, the batch emulation and emu_leaf in tests/emu),
+ * so that every walk -- its operations, its end score and the paths it took -- can be compared between the two and held
+ * against the plain matrix.  aln_leaf fills it through an optional pointer; the counters exist only in these builds. */
+#define ALN_LEAF_REC 1
+struct AlnLeafRec {
+    int32_t aln, r0, c0, n, m;
+    int32_t band;  /* what myers_pass got: -1 none */
+    int32_t top;   /* the rect's flags (ALN_TOP, ALN_GUESS) */
+    int32_t score; /* D at the leaf's last cell as the walk reads it from the records; n + m when n or m is 0 */
+    int32_t diag_rounds, diag_ops, matches; /* rounds that moved diagonally, their moves, the matches among them */
+    int32_t up_rounds, left_rounds;
+    int32_t full_runs;                      /* rounds whose whole diagonal of 32 cells moved diagonally (~dm == 0) */
+    int32_t reload_block, reload_col;       /* window reloads: the walk entered the block above / moved > 24 columns */
+    int32_t border_lanes;                   /* cells rated on the left border (jw - l == 0) */
+    int32_t tail, tail_kind;                /* moves along a border after the walk: 1 insertions, 2 deletions, 0 none */
+    int32_t pad;
+    long long cells;                        /* what myers_pass returned */
+    unsigned long long ops_hash;            /* aln_ops_digest of the leaf's (n + m)-byte region, holes included */
+};
+/* Hash of an operations region: the wrapping sum over positions p of mix64(p << 8 | op), holes (OP_NONE) included,
+ * independent of the order lanes visit the positions in.  Whole warp. */
+POA_FN_NOINLINE unsigned long long aln_ops_digest(const uint8_t* ops, int32_t len) {
+    len = poa_uniform(len);
+    PerLane<unsigned long long> acc;
+    POA_LANES(l) { acc[l] = 0; }
+    for (int32_t base = 0; base < len; base += 32) {
+        POA_LANES(l) {
+            const int32_t p = base + l;
+            if (p < len) acc[l] += aln_mix64((((unsigned long long)(uint32_t)p << 8) | (uint32_t)glb_u8(ops + p)) + 0x9e3779b97f4a7c15ull);
+        }
+    }
+    return aln_warp_sum64(acc);
+}
+/* the walk's record is complete: hash its region, hand it over; whole warp */
+POA_FN void aln_leaf_finish(AlnLeafRec* rec, AlnLeafRec& lr, const uint8_t* ops, int32_t len) {
+    POA_FENCE(); /* the region was written by every lane */
+    lr.ops_hash = aln_ops_digest(ops, len);
+    POA_LANE0 { *rec = lr; }
+    POA_SYNC();
+}
+#define ALN_LEAF_COUNT(stmt) stmt
+#else
+#define ALN_LEAF_REC 0
+#define ALN_LEAF_COUNT(stmt)
 #endif
 
 /* ------------------------------------------------------------------------------------------
@@ -821,12 +874,23 @@ POA_FN void leaf_window_load(const AlnSlot& s, LeafWindow& w, int32_t b, int32_t
  * moves in front of the walk, and the whole run -- matches and mismatches -- is written in one coalesced store.  Up and
  * left moves take a round each.  A new window of records is loaded every 25 columns or when the walk enters the block
  * above.
+ * Test builds (ALN_LEAF_REC): rec (nullable) receives the leaf's AlnLeafRec -- every field but aln, r0, c0 and top.
  */
 POA_FN_NOINLINE int64_t aln_leaf(const AlnSlot& s_ref, EqTab& eq, const uint8_t* q, const uint8_t* t, int32_t n, int32_t m,
-                                 int32_t band, uint8_t* ops, int32_t* score_out) {
+                                 int32_t band, uint8_t* ops, int32_t* score_out
+#if ALN_LEAF_REC
+                                 , AlnLeafRec* rec = nullptr
+#endif
+) {
     const AlnSlot s = s_ref;
     n = poa_uniform(n);
     m = poa_uniform(m);
+#if ALN_LEAF_REC
+    AlnLeafRec lr{};
+    lr.n = n;
+    lr.m = m;
+    lr.band = band;
+#endif
     if (n == 0 || m == 0) { /* edlib.cpp:1135-1142 */
         const int32_t len = n + m;
         const uint8_t op = n == 0 ? OP_DELETE : OP_INSERT;
@@ -839,6 +903,14 @@ POA_FN_NOINLINE int64_t aln_leaf(const AlnSlot& s_ref, EqTab& eq, const uint8_t*
             POA_LANE0 { *score_out = len; }
         }
         POA_SYNC();
+#if ALN_LEAF_REC
+        if (rec) {
+            lr.score = len;
+            lr.tail = len;
+            lr.tail_kind = len == 0 ? 0 : n == 0 ? 2 : 1;
+            aln_leaf_finish(rec, lr, ops, len);
+        }
+#endif
         return 0;
     }
     const int64_t cells = myers_pass<false>(SeqView{q, 1}, n, SeqView{t, 1}, m, band, TeamCtx{0, 1, 0, 0}, s.hbuf, s.hrow_words, s.tcode,
@@ -854,18 +926,26 @@ POA_FN_NOINLINE int64_t aln_leaf(const AlnSlot& s_ref, EqTab& eq, const uint8_t*
             *score_out = win.S[0] - aln_popc64(win.P[0] & aln_below(k)) + aln_popc64(win.M[0] & aln_below(k));
         }
     }
+#if ALN_LEAF_REC
+    POA_LANE0 { lr.score = win.S[0] - aln_popc64(win.P[0] & aln_below(i & 63)) + aln_popc64(win.M[0] & aln_below(i & 63)); }
+#endif
     int32_t w = n + m; /* next write position + 1 */
     while (i >= 0 && j >= 0) {
         if ((i >> 6) != wb || jw - j > 24) { /* the walk left the window, or fewer than 7 cells of its diagonal are in it */
+            ALN_LEAF_COUNT(if ((i >> 6) != wb) ++lr.reload_block; else ++lr.reload_col;)
             wb = i >> 6;
             jw = j;
             leaf_window_load(s, win, wb, jw, B, m);
         }
         const int32_t off = jw - j, k = i & 63;
         PerLane<int> is_diag, is_up, is_match;
+#if ALN_LEAF_REC
+        PerLane<int> on_border;
+#endif
         POA_LANES(l) {
             const int32_t d = l - off, kk = k - d; /* lane l rates cell (i - d, j - d): row kk of the block, column jw - l */
             int diag = 0, up = 0, match = 0;
+            ALN_LEAF_COUNT(on_border[l] = 0;)
             if (d >= 0 && kk >= 0 && jw - l >= 0) {
                 const uint64_t under = aln_below(kk);
                 const int32_t cell = win.S[l] - aln_popc64(win.P[l] & under) + aln_popc64(win.M[l] & under);
@@ -877,6 +957,7 @@ POA_FN_NOINLINE int64_t aln_leaf(const AlnSlot& s_ref, EqTab& eq, const uint8_t*
                 } else { /* the left border: D[r + 1][0] = r + 1 */
                     lf = (i - d) + 1;
                     ul = i - d;
+                    ALN_LEAF_COUNT(on_border[l] = 1;)
                 }
                 if (u + 1 == cell) up = 1;                 /* up: the query character stands alone (edlib.cpp:983-1013) */
                 else if (lf + 1 != cell) diag = 1;          /* not left (:1015-1044) either: diagonal (:1046-1093)        */
@@ -888,11 +969,18 @@ POA_FN_NOINLINE int64_t aln_leaf(const AlnSlot& s_ref, EqTab& eq, const uint8_t*
         }
         const unsigned dm = warp_ballot(is_diag) >> off; /* bit d: the cell d steps down the diagonal moves diagonally */
         const int32_t run = ~dm == 0u ? 32 : poa_ffs(~dm);
+        ALN_LEAF_COUNT(lr.border_lanes += b200poa::poa_popc(warp_ballot(on_border));)
         if (run > 0) {
             POA_LANES(l) {
                 const int32_t d = l - off;
                 if (d >= 0 && d < run) ops[w - 1 - d] = is_match[l] ? OP_MATCH : OP_MISMATCH;
             }
+#if ALN_LEAF_REC
+            ++lr.diag_rounds;
+            lr.diag_ops += run;
+            lr.full_runs += run == 32 ? 1 : 0;
+            lr.matches += b200poa::poa_popc((warp_ballot(is_match) >> off) & (run == 32 ? ~0u : (1u << run) - 1u));
+#endif
             w -= run;
             i -= run;
             j -= run;
@@ -900,6 +988,7 @@ POA_FN_NOINLINE int64_t aln_leaf(const AlnSlot& s_ref, EqTab& eq, const uint8_t*
             const bool up = ((warp_ballot(is_up) >> off) & 1u) != 0u;
             --w;
             POA_LANE0 { ops[w] = up ? OP_INSERT : OP_DELETE; }
+            ALN_LEAF_COUNT(if (up) ++lr.up_rounds; else ++lr.left_rounds;)
             if (up) --i;
             else --j;
         }
@@ -913,6 +1002,14 @@ POA_FN_NOINLINE int64_t aln_leaf(const AlnSlot& s_ref, EqTab& eq, const uint8_t*
         }
     }
     POA_SYNC();
+#if ALN_LEAF_REC
+    if (rec) {
+        lr.tail = rest;
+        lr.tail_kind = rest == 0 ? 0 : i >= 0 ? 1 : 2;
+        lr.cells = cells;
+        aln_leaf_finish(rec, lr, ops, n + m);
+    }
+#endif
     return cells;
 }
 

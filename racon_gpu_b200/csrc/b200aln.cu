@@ -81,6 +81,11 @@ struct AlnKernelArgs {
     int32_t* log_count; /* records appended; more than log_cap: the log overflowed */
     int32_t log_cap;
 #endif
+#if ALN_LEAF_DIGEST
+    AlnLeafRec* leaf_log;    /* [leaf_log_cap] one record per leaf (b200aln_debug_leaf_log) */
+    int32_t* leaf_log_count; /* records appended; more than leaf_log_cap: the log overflowed */
+    int32_t leaf_log_cap;
+#endif
 };
 
 constexpr int WARPS_PER_BLOCK = 2;
@@ -306,11 +311,28 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK, ALN_MIN_BLOCKS) aln_leaf
         if (k >= n_leaves) break;
         const AlnRect r = leaves[k];
         const AlnJob job = a.jobs[r.aln];
+#if ALN_LEAF_DIGEST
+        AlnLeafRec lr;
+#endif
         const int64_t cells = aln_leaf(s, eq, a.seq + job.q_off + r.r0, a.seq + job.t_off + r.c0, r.n, r.m,
                                        (r.top & ALN_GUESS) ? -1 : aln_band_of(r.best), a.ops + job.ops_off + r.r0 + r.c0,
-                                       (r.top & ALN_TOP) ? &a.res[r.aln].score : nullptr);
+                                       (r.top & ALN_TOP) ? &a.res[r.aln].score : nullptr
+#if ALN_LEAF_DIGEST
+                                       , &lr
+#endif
+        );
         if ((threadIdx.x & 31u) == 0u)
             atomicAdd(reinterpret_cast<unsigned long long*>(a.counters + CT_CELLS), (unsigned long long)cells);
+#if ALN_LEAF_DIGEST
+        if ((threadIdx.x & 31u) == 0u) { /* lane 0 holds the record */
+            lr.aln = r.aln;
+            lr.r0 = r.r0;
+            lr.c0 = r.c0;
+            lr.top = r.top;
+            const int32_t at = atomicAdd(a.leaf_log_count, 1);
+            if (at < a.leaf_log_cap) a.leaf_log[at] = lr;
+        }
+#endif
         __syncwarp();
     }
 }
@@ -475,6 +497,10 @@ struct b200aln_batch {
     DevBuf d_log; /* count, then the records of the last align_all (b200aln_debug_split_log) */
     int32_t log_cap = 0;
 #endif
+#if ALN_LEAF_DIGEST
+    DevBuf d_leaf_log; /* count, then the records of the last align_all (b200aln_debug_leaf_log) */
+    int32_t leaf_log_cap = 0;
+#endif
 };
 
 namespace {
@@ -587,6 +613,9 @@ void b200aln_batch_destroy(b200aln_batch* b) {
     b->d_counters.release();
 #if ALN_SPLIT_DIGEST
     b->d_log.release();
+#endif
+#if ALN_LEAF_DIGEST
+    b->d_leaf_log.release();
 #endif
     b->h_seq.release();
     b->h_runs.release();
@@ -789,6 +818,12 @@ int32_t b200aln_batch_align_all(b200aln_batch* b) {
     ALN_CU(b->d_log.need(sizeof(AlnSplitRec) * ((size_t)b->log_cap + 1)));
     ALN_CU(cudaMemsetAsync(b->d_log.p, 0, sizeof(AlnSplitRec), b->stream));
 #endif
+#if ALN_LEAF_DIGEST
+    /* a record per leaf: the leaf list's capacity (more leaves would have overflowed the list itself) */
+    b->leaf_log_cap = (int32_t)std::min<int64_t>(cap_leaves, 0x7FFFFFF);
+    ALN_CU(b->d_leaf_log.need(sizeof(AlnLeafRec) * ((size_t)b->leaf_log_cap + 1)));
+    ALN_CU(cudaMemsetAsync(b->d_leaf_log.p, 0, sizeof(AlnLeafRec), b->stream));
+#endif
 
     cudaStream_t s = b->stream;
     int32_t* ct = static_cast<int32_t*>(b->d_counters.p);
@@ -833,6 +868,11 @@ int32_t b200aln_batch_align_all(b200aln_batch* b) {
     a.log_count = static_cast<int32_t*>(b->d_log.p);
     a.log = static_cast<AlnSplitRec*>(b->d_log.p) + 1;
     a.log_cap = b->log_cap;
+#endif
+#if ALN_LEAF_DIGEST
+    a.leaf_log_count = static_cast<int32_t*>(b->d_leaf_log.p);
+    a.leaf_log = static_cast<AlnLeafRec*>(b->d_leaf_log.p) + 1;
+    a.leaf_log_cap = b->leaf_log_cap;
 #endif
     const int32_t max_blocks = b->n_slots / WARPS_PER_BLOCK;
     auto grid_for = [&](int64_t items) {
@@ -1471,5 +1511,25 @@ extern "C" int32_t b200aln_debug_split_log(b200aln_batch* b, void* out, int64_t 
     if (out && k > 0)
         ALN_CU(cudaMemcpy(out, static_cast<AlnSplitRec*>(b->d_log.p) + 1, sizeof(AlnSplitRec) * (size_t)k, cudaMemcpyDeviceToHost));
     return n > b->log_cap ? B200ALN_GENERIC_ERROR : B200ALN_SUCCESS;
+}
+#endif
+
+#if ALN_LEAF_DIGEST
+/* test build only (not part of include/b200aln.h): the leaf log of the last align_all, one AlnLeafRec per leaf in the
+ * order the leaf kernel appended them.  Same contract as b200aln_debug_split_log. */
+extern "C" int32_t b200aln_debug_leaf_log(b200aln_batch* b, void* out, int64_t cap, int64_t* count, int32_t* rec_bytes) {
+    if (!b || !count) return B200ALN_INVALID_ARGUMENT;
+    if (rec_bytes) *rec_bytes = (int32_t)sizeof(AlnLeafRec);
+    *count = 0;
+    if (!b->aligned || !b->d_leaf_log.p) return B200ALN_UNINITIALIZED;
+    ALN_CU(cudaSetDevice(b->device));
+    ALN_CU(cudaStreamSynchronize(b->stream));
+    int32_t n = 0;
+    ALN_CU(cudaMemcpy(&n, b->d_leaf_log.p, sizeof(int32_t), cudaMemcpyDeviceToHost));
+    *count = n;
+    const int64_t k = std::min<int64_t>(std::min<int64_t>(n, b->leaf_log_cap), cap);
+    if (out && k > 0)
+        ALN_CU(cudaMemcpy(out, static_cast<AlnLeafRec*>(b->d_leaf_log.p) + 1, sizeof(AlnLeafRec) * (size_t)k, cudaMemcpyDeviceToHost));
+    return n > b->leaf_log_cap ? B200ALN_GENERIC_ERROR : B200ALN_SUCCESS;
 }
 #endif

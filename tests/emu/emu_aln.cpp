@@ -305,6 +305,53 @@ int32_t emu_split(const uint8_t* q, int32_t n, const uint8_t* t, int32_t m, int3
     return attempts;
 }
 
+int32_t emu_leaf_rec_bytes(void) { return (int32_t)sizeof(AlnLeafRec); }
+
+/* aln_ops_digest of len bytes (the hash the leaf records carry) */
+uint64_t emu_ops_digest(const uint8_t* ops, int32_t len) { return aln_ops_digest(ops, len); }
+
+/* a slab for one slot of sequences up to max_len, 256-byte aligned like the device's */
+static uint8_t* emu_slot(std::vector<uint8_t>& slab, AlnSlot& s, int32_t max_len, size_t* bytes) {
+    size_t slot_bytes = 0;
+    aln_slot_bind(s, nullptr, max_len, &slot_bytes);
+    slab.assign(slot_bytes + 512, 0);
+    uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(slab.data()) + 255) & ~uintptr_t(255));
+    aln_slot_bind(s, base, max_len, nullptr);
+    if (bytes) *bytes = slot_bytes;
+    return base;
+}
+
+/* One leaf the way aln_leaf_kernel runs it, in a slot whose whole workspace (hand-over row, code row, columns, leaf
+ * records, scores, pre) first holds: poison 0 zeros, 1 0xFF bytes, 2 0xA5 bytes, 3 seeded random bytes, 4 seeded random
+ * bytes and then the leftovers of the leaf (pq, pn, pt, pm) run in it with band pband.  ops_out: the leaf's (n + m)-byte
+ * region, holes OP_NONE; *rec its record (aln, r0, c0, top 0).  Returns the cells the pass computed. */
+int64_t emu_leaf(const uint8_t* q, int32_t n, const uint8_t* t, int32_t m, int32_t band, int32_t poison, uint64_t seed,
+                 const uint8_t* pq, int32_t pn, const uint8_t* pt, int32_t pm, int32_t pband, uint8_t* ops_out, AlnLeafRec* rec) {
+    int32_t max_len = (n > m ? n : m) + 1;
+    if (poison == 4 && (pn > pm ? pn : pm) + 1 > max_len) max_len = (pn > pm ? pn : pm) + 1;
+    std::vector<uint8_t> slab;
+    AlnSlot s;
+    EqTab eq;
+    size_t bytes = 0;
+    uint8_t* base = emu_slot(slab, s, max_len, &bytes);
+    if (poison == 0 || poison == 1 || poison == 2) {
+        std::memset(base, poison == 0 ? 0x00 : poison == 1 ? 0xFF : 0xA5, bytes);
+    } else {
+        std::mt19937_64 rng(seed);
+        for (size_t k = 0; k < bytes; ++k) base[k] = (uint8_t)(rng() >> 56);
+    }
+    if (poison == 4) {
+        std::vector<uint8_t> other((size_t)pn + (size_t)pm + 1, OP_NONE);
+        AlnLeafRec x;
+        aln_leaf(s, eq, pq, pt, pn, pm, pband, other.data(), nullptr, &x);
+    }
+    std::memset(ops_out, OP_NONE, (size_t)n + (size_t)m);
+    std::memset(rec, 0, sizeof *rec);
+    const int64_t cells = aln_leaf(s, eq, q, t, n, m, band, ops_out, nullptr, rec);
+    rec->aln = rec->r0 = rec->c0 = rec->top = 0;
+    return cells;
+}
+
 /* Aligns one pair; ops_out must hold n + m bytes.  Returns the number of operations (holes removed); -1 inconsistent
  * split, -2 list overflow, -3 the runs do not spell the operations.  *score the edit distance; *levels (nullable) the
  * depth of the recursion; *n_leaves likewise; cigar_out (nullable, cigar_cap bytes) the CIGAR formed from the runs;
@@ -312,11 +359,13 @@ int32_t emu_split(const uint8_t* q, int32_t n, const uint8_t* t, int32_t m, int3
  * guess (< 0: none) a guessed bound on the edit distance: the top sub-problem runs banded and is redone without a band when
  * its optimum turns out larger (what the kernels do with the host's guess).  log (nullable, log_cap records): one record
  * per split attempt like the device's split log (b200aln_debug_split_log), alignment index aln_index, path one warp;
- * *log_count = records written (more than log_cap: the rest were dropped). */
+ * *log_count = records written (more than log_cap: the rest were dropped).  leaf_log (nullable, leaf_cap records): one
+ * record per leaf like the device's leaf log (b200aln_debug_leaf_log); *leaf_count = leaves. */
 int64_t emu_align(const uint8_t* q, int32_t n, const uint8_t* t, int32_t m, uint8_t* ops_out, int32_t* score,
                   int32_t* levels, int32_t* n_leaves, char* cigar_out, int64_t cigar_cap, int32_t q_first, int32_t t_begin,
                   int32_t window_length, uint32_t* bp_out, int32_t* bp_count, int32_t guess, int32_t aln_index,
-                  AlnSplitRec* log, int64_t log_cap, int64_t* log_count) {
+                  AlnSplitRec* log, int64_t log_cap, int64_t* log_count, AlnLeafRec* leaf_log, int64_t leaf_cap,
+                  int64_t* leaf_count) {
     const int32_t max_len = (n > m ? n : m) + 1;
     size_t slot_bytes = 0;
     AlnSlot s;
@@ -378,9 +427,16 @@ int64_t emu_align(const uint8_t* q, int32_t n, const uint8_t* t, int32_t m, uint
     if (overflow) return -2;
     for (int32_t k = 0; k < n_leaf; ++k) {
         const AlnRect r = leaves[(size_t)k];
+        AlnLeafRec x;
         aln_leaf(s, eq, q + r.r0, t + r.c0, r.n, r.m, (r.top & ALN_GUESS) ? -1 : aln_band_of(r.best), ops.data() + r.r0 + r.c0,
-                 (r.top & ALN_TOP) ? score : nullptr);
+                 (r.top & ALN_TOP) ? score : nullptr, &x);
+        x.aln = r.aln;
+        x.r0 = r.r0;
+        x.c0 = r.c0;
+        x.top = r.top;
+        if (leaf_log && k < leaf_cap) leaf_log[k] = x;
     }
+    if (leaf_count) *leaf_count = n_leaf;
     int64_t k = 0;
     for (uint8_t op : ops)
         if (op != OP_NONE) ops_out[k++] = op;

@@ -127,7 +127,8 @@ class EmuAligner:
         n = self.lib.emu_align(C.c_char_p(q), C.c_int32(len(q)), C.c_char_p(t), C.c_int32(len(t)), _p(ops, C.c_uint8),
                                C.byref(score), C.byref(levels), C.byref(leaves), cigar, C.c_int64(cap),
                                C.c_int32(q_first), C.c_int32(t_begin), C.c_int32(window_length), _p(bp, C.c_uint32),
-                               C.byref(bp_count), C.c_int32(guess), C.c_int32(0), None, C.c_int64(0), None)
+                               C.byref(bp_count), C.c_int32(guess), C.c_int32(0), None, C.c_int64(0), None, None,
+                               C.c_int64(0), None)
         self.breaking_points = bp[:2 * bp_count.value].reshape(-1, 2).copy()  # (t, q) pairs, window_length > 0 only
         assert n >= 0, {-1: "inconsistent split", -2: "list overflow", -3: "runs do not spell the operations"}.get(n, n)
         self.cigar = cigar.value
@@ -146,9 +147,49 @@ class EmuAligner:
         n = self.lib.emu_align(C.c_char_p(q), C.c_int32(len(q)), C.c_char_p(t), C.c_int32(len(t)), _p(ops, C.c_uint8),
                                C.byref(score), None, None, None, C.c_int64(0), C.c_int32(0), C.c_int32(0), C.c_int32(0),
                                None, None, C.c_int32(guess), C.c_int32(aln), log.ctypes.data_as(C.c_void_p),
-                               C.c_int64(cap), C.byref(count))
+                               C.c_int64(cap), C.byref(count), None, C.c_int64(0), None)
         assert n >= 0 and count.value <= cap, (n, count.value, cap)
         return log[:count.value].copy()
+
+    def align_leaves(self, q: bytes, t: bytes, guess: int = -1, aln: int = 0):
+        """The leaf records (racon_gpu_b200.aligner.LEAF_REC_DTYPE) of aligning one pair as alignment `aln` of a batch,
+        in the order the leaf list holds them, and the edit distance."""
+        from racon_gpu_b200.aligner import LEAF_REC_DTYPE
+        assert self.lib.emu_leaf_rec_bytes() == LEAF_REC_DTYPE.itemsize
+        cap = 2 * (len(q) * len(t) // (1 << 19) + len(q) + len(t)) // 64 + 64
+        log = np.zeros(cap, dtype=LEAF_REC_DTYPE)
+        count = C.c_int64(0)
+        ops = np.zeros(len(q) + len(t) + 8, dtype=np.uint8)
+        score = C.c_int32(-1)
+        n = self.lib.emu_align(C.c_char_p(q), C.c_int32(len(q)), C.c_char_p(t), C.c_int32(len(t)), _p(ops, C.c_uint8),
+                               C.byref(score), None, None, None, C.c_int64(0), C.c_int32(0), C.c_int32(0), C.c_int32(0),
+                               None, None, C.c_int32(guess), C.c_int32(aln), None, C.c_int64(0), None,
+                               log.ctypes.data_as(C.c_void_p), C.c_int64(cap), C.byref(count))
+        assert n >= 0 and count.value <= cap, (n, count.value, cap)
+        return log[:count.value].copy(), int(score.value)
+
+    #: emu_leaf's slot contents before the pass: zeros, 0xFF, 0xA5, seeded random bytes, another leaf's leftovers
+    POISONS = ("zero", "ff", "a5", "random", "leftovers")
+
+    def leaf(self, q: bytes, t: bytes, band: int, poison: str = "zero", seed: int = 0, other=None):
+        """One leaf the way aln_leaf_kernel runs it, in a slot filled per `poison` first (other = (q, t, band) of the leaf
+        whose leftovers the slot holds).  Returns (the (n + m)-byte operations region, the LEAF_REC_DTYPE record)."""
+        from racon_gpu_b200.aligner import LEAF_REC_DTYPE
+        self.lib.emu_leaf.restype = C.c_int64
+        region = np.zeros(len(q) + len(t) + 1, dtype=np.uint8)
+        rec = np.zeros(1, dtype=LEAF_REC_DTYPE)
+        pq, pt, pband = other if other is not None else (b"", b"", -1)
+        self.lib.emu_leaf(C.c_char_p(q), C.c_int32(len(q)), C.c_char_p(t), C.c_int32(len(t)), C.c_int32(band),
+                          C.c_int32(self.POISONS.index(poison)), C.c_uint64(seed), C.c_char_p(pq), C.c_int32(len(pq)),
+                          C.c_char_p(pt), C.c_int32(len(pt)), C.c_int32(pband), _p(region, C.c_uint8),
+                          rec.ctypes.data_as(C.c_void_p))
+        return region[:len(q) + len(t)].copy(), rec[0]
+
+    def ops_digest(self, region: np.ndarray) -> int:
+        """aln_ops_digest of an operations region (holes 0xFF included)."""
+        self.lib.emu_ops_digest.restype = C.c_uint64
+        region = np.ascontiguousarray(region, dtype=np.uint8)
+        return int(self.lib.emu_ops_digest(_p(region, C.c_uint8), C.c_int32(region.shape[0])))
 
     #: emu_split's stats, in order
     SPLIT_STATS = ("stripes", "left_matrix", "anchors", "other", "waits", "failures", "timeouts")
