@@ -13,7 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb200poa.so")
 SOURCES = ["b200poa.cu", "b200aln.cu", "host/cuda_batch.cpp", "host/cuda_polisher.cpp"]
-HEADERS = ["poa_core.cuh", "poa_fill.cuh", "poa_simt.cuh", "host/b200_window.hpp", "host/cuda_batch.hpp",
+HEADERS = ["poa_core.cuh", "poa_fill.cuh", "poa_simt.cuh", "cuda_buffers.hpp", "host/b200_window.hpp", "host/cuda_batch.hpp",
            "host/cuda_polisher.hpp", "host/b200poa_batch.hpp", "host/window_arena.hpp", "../../include/b200poa.h",
            "aln_core.cuh", "host/aln_levels.hpp", "host/b200aln_aligner.hpp", "../../include/b200aln.h"]
 

@@ -31,9 +31,11 @@
 
 #include "../../include/b200aln.h"
 #include "aln_core.cuh"
+#include "cuda_buffers.hpp"
 #include "host/aln_levels.hpp"
 
 using namespace b200aln;
+using namespace b200buf;
 
 namespace {
 
@@ -403,51 +405,11 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) aln_cigar_kernel(const A
     }
 }
 
+} // namespace
+
 /* ------------------------------------------------------------------------------------------ */
 /* host side                                                                                   */
 /* ------------------------------------------------------------------------------------------ */
-struct DevBuf { /* grow-only device buffer */
-    void* p = nullptr;
-    size_t cap = 0;
-    cudaError_t need(size_t bytes, bool slack = true) {
-        if (bytes <= cap) return cudaSuccess;
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
-        const size_t want = bytes + (slack ? bytes / 4 : 0) + 256;
-        cudaError_t e = cudaMalloc(&p, want);
-        if (e == cudaSuccess) cap = want;
-        return e;
-    }
-    void release() {
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
-    }
-};
-struct PinnedBuf { /* grow-only page-locked host buffer, contents preserved */
-    uint8_t* p = nullptr;
-    size_t cap = 0, used = 0;
-    bool reserve(size_t bytes) {
-        if (bytes <= cap) return true;
-        size_t want = std::max<size_t>(bytes, cap * 2);
-        want = std::max<size_t>(want, (size_t)1 << 20);
-        uint8_t* q = nullptr;
-        if (cudaHostAlloc(reinterpret_cast<void**>(&q), want, cudaHostAllocDefault) != cudaSuccess) return false;
-        if (used) std::memcpy(q, p, used);
-        if (p) cudaFreeHost(p);
-        p = q;
-        cap = want;
-        return true;
-    }
-    void release() {
-        if (p) cudaFreeHost(p);
-        p = nullptr;
-        cap = used = 0;
-    }
-};
-
-} // namespace
 
 struct b200aln_batch {
     int32_t device = 0;
@@ -489,7 +451,7 @@ struct b200aln_batch {
     bool runs_on_host = false; /* the run starts are fetched only when a caller asks for operations */
     std::vector<int64_t> t_off; /* per alignment, for b200aln_batch_get_cigars */
     std::vector<int32_t> t_len, t_ed, t_st;
-    int32_t* h_counters = nullptr; /* pinned, CT_WORDS */
+    PinnedBuf h_counters; /* CT_WORDS int32 */
     bool aligned = false, synced = false;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     b200aln_batch_info info{};
@@ -589,44 +551,17 @@ const char* b200aln_status_string(int32_t st) {
 void b200aln_batch_destroy(b200aln_batch* b) {
     if (!b) return;
     cudaSetDevice(b->device);
+    /* both streams are idle before the members' destructors free the buffers they used */
     if (b->stream) cudaStreamSynchronize(b->stream);
-    b->d_slab.release();
-    b->d_seq.release();
-    b->d_jobs.release();
-    b->d_ops.release();
-    b->d_res.release();
-    b->d_runs.release();
-    b->d_text.release();
-    b->d_bp.release();
-    for (int c = 0; c < ALN_CLASSES; ++c) {
-        b->d_list[c][0].release();
-        b->d_list[c][1].release();
-    }
-    b->d_team_slab.release();
+    if (b->side) cudaStreamSynchronize(b->side);
     if (b->ev_fork) cudaEventDestroy(b->ev_fork);
     if (b->ev_join) cudaEventDestroy(b->ev_join);
-    if (b->side) {
-        cudaStreamSynchronize(b->side);
-        cudaStreamDestroy(b->side);
-    }
-    b->d_leaves.release();
-    b->d_counters.release();
-#if ALN_SPLIT_DIGEST
-    b->d_log.release();
-#endif
-#if ALN_LEAF_DIGEST
-    b->d_leaf_log.release();
-#endif
-    b->h_seq.release();
-    b->h_runs.release();
-    b->h_text.release();
-    b->h_bp.release();
-    if (b->h_counters) cudaFreeHost(b->h_counters);
+    if (b->side) cudaStreamDestroy(b->side);
     if (b->ev0) cudaEventDestroy(b->ev0);
     if (b->ev1) cudaEventDestroy(b->ev1);
     if (b->own_stream && b->stream) cudaStreamDestroy(b->stream);
-    cudaGetLastError();
     delete b;
+    cudaGetLastError();
 }
 
 int32_t b200aln_batch_create(int32_t device_id, void* stream, int64_t max_gpu_mem, int32_t max_bandwidth,
@@ -672,7 +607,7 @@ int32_t b200aln_batch_create(int32_t device_id, void* stream, int64_t max_gpu_me
             break;
         }
         b->team_blocks_per_sm = std::max(0, bps_team);
-        if (cudaHostAlloc(reinterpret_cast<void**>(&b->h_counters), CT_WORDS * sizeof(int32_t), cudaHostAllocDefault) != cudaSuccess ||
+        if (!b->h_counters.reserve(CT_WORDS * sizeof(int32_t)) ||
             cudaEventCreate(&b->ev0) != cudaSuccess || cudaEventCreate(&b->ev1) != cudaSuccess ||
             cudaStreamCreateWithFlags(&b->side, cudaStreamNonBlocking) != cudaSuccess ||
             cudaEventCreateWithFlags(&b->ev_fork, cudaEventDisableTiming) != cudaSuccess ||
@@ -827,10 +762,11 @@ int32_t b200aln_batch_align_all(b200aln_batch* b) {
 
     cudaStream_t s = b->stream;
     int32_t* ct = static_cast<int32_t*>(b->d_counters.p);
-    std::memset(b->h_counters, 0, sizeof(int32_t) * CT_WORDS);
-    for (int c = 0; c < ALN_CLASSES; ++c) b->h_counters[CT_NOPEN + c] = (int32_t)first[c].size();
-    b->h_counters[CT_NLEAVES] = (int32_t)leaves0.size();
-    ALN_CU(cudaMemcpyAsync(ct, b->h_counters, sizeof(int32_t) * CT_WORDS, cudaMemcpyHostToDevice, s));
+    int32_t* hc = reinterpret_cast<int32_t*>(b->h_counters.p);
+    std::memset(hc, 0, sizeof(int32_t) * CT_WORDS);
+    for (int c = 0; c < ALN_CLASSES; ++c) hc[CT_NOPEN + c] = (int32_t)first[c].size();
+    hc[CT_NLEAVES] = (int32_t)leaves0.size();
+    ALN_CU(cudaMemcpyAsync(ct, hc, sizeof(int32_t) * CT_WORDS, cudaMemcpyHostToDevice, s));
     if (b->view_q) { /* straight from the caller's buffers (page-locked ones upload at full PCIe speed) */
         if (b->view_q_bytes)
             ALN_CU(cudaMemcpyAsync(b->d_seq.p, b->view_q, (size_t)b->view_q_bytes, cudaMemcpyHostToDevice, s));
@@ -953,18 +889,18 @@ int32_t b200aln_batch_align_all(b200aln_batch* b) {
         ALN_CU(cudaGetLastError());
         if (forked) ALN_CU(cudaStreamWaitEvent(s, b->ev_join, 0));
         b->info.n_open += (int64_t)n_open[0] + n_open[1] + n_open[2];
-        ALN_CU(cudaMemcpyAsync(b->h_counters + CT_NOPEN + 4 * (level + 1), ct_next, ALN_CLASSES * sizeof(int32_t),
+        ALN_CU(cudaMemcpyAsync(hc + CT_NOPEN + 4 * (level + 1), ct_next, ALN_CLASSES * sizeof(int32_t),
                                cudaMemcpyDeviceToHost, s));
         ALN_CU(cudaStreamSynchronize(s));
         for (int c = 0; c < ALN_CLASSES; ++c)
-            n_open[c] = std::min<int32_t>(b->h_counters[CT_NOPEN + 4 * (level + 1) + c], (int32_t)cap_open);
+            n_open[c] = std::min<int32_t>(hc[CT_NOPEN + 4 * (level + 1) + c], (int32_t)cap_open);
         ++level;
     }
     b->info.levels = level;
-    ALN_CU(cudaMemcpyAsync(b->h_counters + CT_NLEAVES, ct + CT_NLEAVES, 2 * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    ALN_CU(cudaMemcpyAsync(hc + CT_NLEAVES, ct + CT_NLEAVES, 2 * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
     ALN_CU(cudaStreamSynchronize(s));
-    if (b->h_counters[CT_OVERFLOW]) return B200ALN_GENERIC_ERROR;
-    const int32_t n_leaves = b->h_counters[CT_NLEAVES];
+    if (hc[CT_OVERFLOW]) return B200ALN_GENERIC_ERROR;
+    const int32_t n_leaves = hc[CT_NLEAVES];
     b->info.n_leaves = n_leaves;
     if (n_leaves > 0) {
         aln_leaf_kernel<<<grid_for(n_leaves), 32 * WARPS_PER_BLOCK, 0, s>>>(a, static_cast<const AlnRect*>(b->d_leaves.p),
@@ -988,12 +924,12 @@ int32_t b200aln_batch_align_all(b200aln_batch* b) {
     /* compact results: the per-alignment records and the counters now, then exactly the CIGAR bytes produced; the run
      * starts stay on the device until a caller asks for operations (b200aln_batch_get_alignment / _get_ops) */
     ALN_CU(cudaMemcpyAsync(b->res.data(), b->d_res.p, sizeof(AlnResult) * (size_t)n_aln, cudaMemcpyDeviceToHost, s));
-    ALN_CU(cudaMemcpyAsync(b->h_counters + CT_RUNS, ct + CT_RUNS, 10 * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    ALN_CU(cudaMemcpyAsync(hc + CT_RUNS, ct + CT_RUNS, 10 * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
     ALN_CU(cudaStreamSynchronize(s));
     unsigned long long n_runs_total = 0, cells = 0, text_total = 0;
-    std::memcpy(&n_runs_total, b->h_counters + CT_RUNS, 8);
-    std::memcpy(&cells, b->h_counters + CT_CELLS, 8);
-    std::memcpy(&text_total, b->h_counters + CT_TEXT, 8);
+    std::memcpy(&n_runs_total, hc + CT_RUNS, 8);
+    std::memcpy(&cells, hc + CT_CELLS, 8);
+    std::memcpy(&text_total, hc + CT_TEXT, 8);
     b->info.cells = (int64_t)cells;
     b->n_runs_total = std::min<unsigned long long>(n_runs_total, (unsigned long long)b->ops_bytes + 64);
     text_total = std::min<unsigned long long>(text_total, text_cap);
@@ -1002,7 +938,7 @@ int32_t b200aln_batch_align_all(b200aln_batch* b) {
     if (text_total)
         ALN_CU(cudaMemcpyAsync(b->h_text.p, b->d_text.p, (size_t)text_total, cudaMemcpyDeviceToHost, s));
     unsigned long long bp_total = 0;
-    std::memcpy(&bp_total, b->h_counters + CT_BP, 8);
+    std::memcpy(&bp_total, hc + CT_BP, 8);
     bp_total = want_bp ? std::min<unsigned long long>(bp_total, bp_cap) : 0;
     if (!b->h_bp.reserve((size_t)bp_total * 8 + 64)) return B200ALN_GENERIC_ERROR;
     b->h_bp.used = (size_t)bp_total * 8;

@@ -20,6 +20,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <new>
 #include <numeric>
 #include <vector>
@@ -27,8 +28,10 @@
 #include "../../include/b200poa.h"
 #include "poa_core.cuh"
 #include "poa_fill.cuh"
+#include "cuda_buffers.hpp"
 
 using namespace b200poa;
+using namespace b200buf;
 
 /* ------------------------------------------------------------------------------------------ */
 /* kernel                                                                                      */
@@ -194,24 +197,12 @@ __global__ void __launch_bounds__(32, POA_MIN_BLOCKS_PER_SM) poa_window_kernel(c
     } while (0)
 
 namespace {
-
 std::atomic<int32_t> g_batches{0};
-
-struct DeviceGuard { /* scoped_device_switch (GenomeWorks common/base cudautils.hpp) */
-    int prev = -1;
-    explicit DeviceGuard(int dev) {
-        cudaGetDevice(&prev);
-        if (prev != dev) cudaSetDevice(dev);
-        else prev = -1;
-    }
-    ~DeviceGuard() {
-        if (prev >= 0) cudaSetDevice(prev);
-    }
-};
-
 } // namespace
 
+/* Every buffer is a member that frees itself (cuda_buffers.hpp); the destructor waits for the batch's stream first. */
 struct b200poa_batch {
+    ~b200poa_batch() { cudaStreamSynchronize(stream); }
     int32_t id = 0;
     int32_t device = 0;
     cudaStream_t stream = nullptr;
@@ -232,76 +223,36 @@ struct b200poa_batch {
     int32_t sm_count = 0;
     int32_t max_len_staged = 0;
     size_t device_bytes = 0;
-    /* pinned host staging */
-    uint8_t* h_bases = nullptr;
-    int8_t* h_weights = nullptr;
-    int64_t* h_seq_off = nullptr;
-    int64_t* h_w_off = nullptr;
-    int32_t* h_seq_len = nullptr;
-    int32_t* h_seq_begin = nullptr;
-    int32_t* h_seq_end = nullptr;
-    int32_t* h_win_seq_off = nullptr;
-    int32_t* h_win_flags = nullptr;
-    int32_t* h_win_trim_nseq = nullptr;
-    int32_t* h_work = nullptr;
-    uint8_t* h_cons = nullptr;
-    uint16_t* h_cov = nullptr;
-    int32_t* h_len = nullptr;
-    int32_t* h_status = nullptr;
-    int32_t* h_out_off = nullptr;
-    int32_t* h_trim = nullptr;
-    int32_t* h_cursor = nullptr; /* [2] as on the device */
-    /* device */
-    uint8_t* d_slab = nullptr;
-    uint8_t* d_bases = nullptr;
-    int8_t* d_weights = nullptr;
-    int64_t* d_seq_off = nullptr;
-    int64_t* d_w_off = nullptr;
-    int32_t* d_seq_len = nullptr;
-    int32_t* d_seq_begin = nullptr;
-    int32_t* d_seq_end = nullptr;
-    int32_t* d_win_seq_off = nullptr;
-    int32_t* d_win_flags = nullptr;
-    int32_t* d_win_trim_nseq = nullptr;
-    int32_t* d_work = nullptr;
-    int32_t* d_cursor = nullptr;
-    uint8_t* d_cons = nullptr;
-    uint16_t* d_cov = nullptr;
-    int32_t* d_len = nullptr;
-    int32_t* d_status = nullptr;
-    int32_t* d_out_off = nullptr;
-    int32_t* d_trim = nullptr;
-    unsigned long long* d_phase = nullptr; /* B200POA_PHASE_TIMERS diagnostics */
+    /* staged inputs (pinned host -> device); in direct mode bases and weights go up from the caller's arena instead */
+    Mirror<uint8_t> bases;
+    Mirror<int8_t> weights;
+    Mirror<int64_t> seq_off, w_off;
+    Mirror<int32_t> seq_len, seq_begin, seq_end;
+    Mirror<int32_t> win_seq_off, win_flags, win_trim_nseq, work;
+    /* outputs (device -> pinned host) */
+    Mirror<int32_t> cursor; /* [2] work cursor, elements used in the output arenas */
+    Mirror<uint8_t> cons;
+    Mirror<uint16_t> cov;
+    Mirror<int32_t> len, status, out_off, trim;
+    DevBuf slab;
+    DevBuf phase; /* B200POA_PHASE_TIMERS diagnostics */
     /* multiple sequence alignment (output mask has B200POA_OUTPUT_MSA) */
-    uint16_t* d_path = nullptr;            /* [arena_cap] node of every base */
-    uint8_t* d_msa = nullptr;              /* [msa_cap] compact rows */
-    unsigned long long* d_msa_cursor = nullptr;
-    long long* d_msa_off = nullptr;
-    int32_t* d_msa_cols = nullptr;
-    int32_t* d_msa_status = nullptr;
-    uint8_t* h_msa = nullptr;              /* pinned, grown on demand to the bytes a launch used */
-    size_t h_msa_bytes = 0;
-    unsigned long long* h_msa_cursor = nullptr;
-    long long* h_msa_off = nullptr;
-    int32_t* h_msa_cols = nullptr;
-    int32_t* h_msa_status = nullptr;
-    int32_t* h_msa_rows = nullptr;         /* sequences staged per window = rows of its MSA */
+    DevBuf path;                        /* [arena_cap] node of every base */
+    DevBuf msa;                         /* [msa_cap] compact rows */
+    Mirror<unsigned long long> msa_cursor;
+    Mirror<long long> msa_off;
+    Mirror<int32_t> msa_cols, msa_status;
+    PinnedBuf h_msa;                    /* grown on demand to the bytes a launch used */
+    PinnedBuf h_msa_rows;               /* int32 per window: sequences staged = rows of its MSA */
 #if POA_FILL_DIGEST
-    unsigned long long* d_fill_digest = nullptr; /* [max_seqs] per staged sequence, see b200poa_debug_fill_digest */
-    int32_t* d_fill_count = nullptr;
+    DevBuf fill_digest, fill_count; /* [max_seqs] per staged sequence, see b200poa_debug_fill_digest */
 #endif
 #if POA_ALN_DIGEST
-    unsigned long long* d_aln_digest = nullptr; /* [max_seqs] see b200poa_debug_aln_digest */
-    int32_t* d_aln_count = nullptr;
+    DevBuf aln_digest, aln_count; /* [max_seqs] see b200poa_debug_aln_digest */
 #endif
 #if POA_GRAPH_DIGEST
-    unsigned long long* d_graph_digest = nullptr; /* [max_seqs] see b200poa_debug_graph_digest */
-    int32_t* d_graph_nodes = nullptr;
-    int32_t* d_graph_edges = nullptr;
-    unsigned long long* d_sub_digest = nullptr;
-    int32_t* d_sub_count = nullptr;
-    unsigned long long* d_cons_digest = nullptr; /* [2 x max_poas] */
-    int32_t* d_cons_rounds = nullptr;            /* [max_poas] */
+    DevBuf graph_digest, graph_nodes, graph_edges, sub_digest, sub_count; /* [max_seqs] see b200poa_debug_graph_digest */
+    DevBuf cons_digest, cons_rounds;                                      /* [2 x max_poas], [max_poas] */
 #endif
     size_t msa_cap = 0;
     size_t msa_bound = 0;                  /* worst-case MSA bytes of the windows staged so far */
@@ -360,79 +311,6 @@ static SmemGeometry smem_geometry(const Params& p, int32_t max_len) {
                                      (g.ring_rows * g.ring_stride + slack_cells) * (int32_t)sizeof(int16_t),
                                  (int32_t)TB_SCRATCH_BYTES);
     return g;
-}
-
-static void free_batch(b200poa_batch* b) {
-    if (!b) return;
-    DeviceGuard g(b->device);
-    cudaFreeHost(b->h_bases);
-    cudaFreeHost(b->h_weights);
-    cudaFreeHost(b->h_seq_off);
-    cudaFreeHost(b->h_w_off);
-    cudaFreeHost(b->h_seq_len);
-    cudaFreeHost(b->h_seq_begin);
-    cudaFreeHost(b->h_seq_end);
-    cudaFreeHost(b->h_win_seq_off);
-    cudaFreeHost(b->h_win_flags);
-    cudaFreeHost(b->h_win_trim_nseq);
-    cudaFreeHost(b->h_work);
-    cudaFreeHost(b->h_cons);
-    cudaFreeHost(b->h_cov);
-    cudaFreeHost(b->h_len);
-    cudaFreeHost(b->h_status);
-    cudaFreeHost(b->h_out_off);
-    cudaFreeHost(b->h_trim);
-    cudaFreeHost(b->h_cursor);
-    cudaFree(b->d_slab);
-    cudaFree(b->d_bases);
-    cudaFree(b->d_weights);
-    cudaFree(b->d_seq_off);
-    cudaFree(b->d_w_off);
-    cudaFree(b->d_seq_len);
-    cudaFree(b->d_seq_begin);
-    cudaFree(b->d_seq_end);
-    cudaFree(b->d_win_seq_off);
-    cudaFree(b->d_win_flags);
-    cudaFree(b->d_win_trim_nseq);
-    cudaFree(b->d_work);
-    cudaFree(b->d_cursor);
-    cudaFree(b->d_cons);
-    cudaFree(b->d_cov);
-    cudaFree(b->d_len);
-    cudaFree(b->d_status);
-    cudaFree(b->d_out_off);
-    cudaFree(b->d_trim);
-    cudaFree(b->d_phase);
-    cudaFree(b->d_path);
-    cudaFree(b->d_msa);
-    cudaFree(b->d_msa_cursor);
-    cudaFree(b->d_msa_off);
-    cudaFree(b->d_msa_cols);
-    cudaFree(b->d_msa_status);
-    cudaFreeHost(b->h_msa);
-    cudaFreeHost(b->h_msa_cursor);
-    cudaFreeHost(b->h_msa_off);
-    cudaFreeHost(b->h_msa_cols);
-    cudaFreeHost(b->h_msa_status);
-    cudaFreeHost(b->h_msa_rows);
-#if POA_FILL_DIGEST
-    cudaFree(b->d_fill_digest);
-    cudaFree(b->d_fill_count);
-#endif
-#if POA_ALN_DIGEST
-    cudaFree(b->d_aln_digest);
-    cudaFree(b->d_aln_count);
-#endif
-#if POA_GRAPH_DIGEST
-    cudaFree(b->d_graph_digest);
-    cudaFree(b->d_graph_nodes);
-    cudaFree(b->d_graph_edges);
-    cudaFree(b->d_sub_digest);
-    cudaFree(b->d_sub_count);
-    cudaFree(b->d_cons_digest);
-    cudaFree(b->d_cons_rounds);
-#endif
-    delete b;
 }
 
 /* One sequence as the staging code sees it. */
@@ -518,14 +396,14 @@ static int32_t stage_window(b200poa_batch* b, int32_t n, Get get, int32_t* per_s
                 if (bg < 0 || en >= bb_len || bg >= en) flag = B200POA_INVALID_ARGUMENT; /* window.cpp:55-59 rejects it */
             }
         }
-        b->h_seq_begin[b->seq_count] = sp_b;
-        b->h_seq_end[b->seq_count] = sp_e;
+        b->seq_begin.h()[b->seq_count] = sp_b;
+        b->seq_end.h()[b->seq_count] = sp_e;
         if (len > b->max_len_staged) b->max_len_staged = len;
         /* weights: a sequence whose bases all weigh the same (no quality string => 1, cudapoa_batch.cuh:525-530;
          * the '!' dummy quality of a FASTA target => 0) ships only that constant */
         int64_t wo = -1 - 1;
         if (DIRECT) {
-            b->h_seq_off[b->seq_count] = q.host_off - b->ext_lo;
+            b->seq_off.h()[b->seq_count] = q.host_off - b->ext_lo;
             if (q.w) {
                 wo = q.wmode;
                 if (wo >= 0) { /* explicit weights: the weights arena mirrors the same host range */
@@ -534,8 +412,8 @@ static int32_t stage_window(b200poa_batch* b, int32_t n, Get get, int32_t* per_s
                 }
             }
         } else {
-            b->h_seq_off[b->seq_count] = b->base_count;
-            std::memcpy(b->h_bases + b->base_count, q.seq, (size_t)len);
+            b->seq_off.h()[b->seq_count] = b->base_count;
+            std::memcpy(b->bases.h() + b->base_count, q.seq, (size_t)len);
             if (q.w) {
                 bool constant = true;
                 for (int32_t k = 1; k < len && constant; ++k) constant = q.w[k] == q.w[0];
@@ -543,25 +421,25 @@ static int32_t stage_window(b200poa_batch* b, int32_t n, Get get, int32_t* per_s
                     wo = -1 - (int64_t)q.w[0];
                 } else {
                     wo = b->weight_count;
-                    std::memcpy(b->h_weights + b->weight_count, q.w, (size_t)len);
+                    std::memcpy(b->weights.h() + b->weight_count, q.w, (size_t)len);
                     b->weight_count += len;
                 }
             }
             b->base_count += len;
         }
-        b->h_w_off[b->seq_count] = wo;
-        b->h_seq_len[b->seq_count] = len;
+        b->w_off.h()[b->seq_count] = wo;
+        b->seq_len.h()[b->seq_count] = len;
         b->seq_count += 1;
         cost += (int64_t)len * (bb_len + (int64_t)added * (bb_len / 8 + 1));
         ++added;
     }
     if (backbone_rejected) flag = B200POA_EXCEEDED_MAXIMUM_SEQUENCE_SIZE; /* the kernel skips the window and reports why */
-    b->h_win_flags[b->poa_count] = flag;
-    b->h_win_trim_nseq[b->poa_count] = b->trim_counts_staged ? added : n; /* window.cpp:121 counts every sequence */
-    if (b->h_msa_rows) b->h_msa_rows[b->poa_count] = added;
+    b->win_flags.h()[b->poa_count] = flag;
+    b->win_trim_nseq.h()[b->poa_count] = b->trim_counts_staged ? added : n; /* window.cpp:121 counts every sequence */
+    if (b->h_msa_rows.p) reinterpret_cast<int32_t*>(b->h_msa_rows.p)[b->poa_count] = added;
     b->msa_bound += msa_need;
     b->poa_count += 1;
-    b->h_win_seq_off[b->poa_count] = (int32_t)b->seq_count;
+    b->win_seq_off.h()[b->poa_count] = (int32_t)b->seq_count;
     b->cost.push_back(cost);
     b->uploaded = false;
     if (n_added_out) *n_added_out = added > 0 ? added - 1 : 0;
@@ -571,80 +449,59 @@ static int32_t stage_window(b200poa_batch* b, int32_t n, Get get, int32_t* per_s
 static int32_t alloc_batch_memory(b200poa_batch* b) {
     const Params& p = b->p;
     const size_t MP = (size_t)b->max_poas, MS = (size_t)b->max_seqs, AC = (size_t)b->arena_cap;
-    CU_TRY(cudaMalloc(&b->d_slab, (size_t)b->n_slots * b->slot_bytes));
+    CU_TRY(b->slab.need((size_t)b->n_slots * b->slot_bytes, false));
     if (const char* env = std::getenv("B200POA_SLAB_FILL")) /* debugging: the engine must not depend on what a slot held before */
-        CU_TRY(cudaMemset(b->d_slab, std::atoi(env), (size_t)b->n_slots * b->slot_bytes));
-    CU_TRY(cudaMalloc(&b->d_bases, AC));
-    CU_TRY(cudaMalloc(&b->d_weights, AC));
-    CU_TRY(cudaMalloc(&b->d_seq_off, (MS + 1) * sizeof(int64_t)));
-    CU_TRY(cudaMalloc(&b->d_w_off, (MS + 1) * sizeof(int64_t)));
-    CU_TRY(cudaMalloc(&b->d_seq_len, (MS + 1) * sizeof(int32_t)));
-    CU_TRY(cudaMalloc(&b->d_seq_begin, (MS + 1) * sizeof(int32_t)));
-    CU_TRY(cudaMalloc(&b->d_seq_end, (MS + 1) * sizeof(int32_t)));
-    CU_TRY(cudaMalloc(&b->d_win_seq_off, (MP + 1) * sizeof(int32_t)));
-    CU_TRY(cudaMalloc(&b->d_win_flags, MP * sizeof(int32_t)));
-    CU_TRY(cudaMalloc(&b->d_win_trim_nseq, MP * sizeof(int32_t)));
-    CU_TRY(cudaMalloc(&b->d_work, MP * sizeof(int32_t)));
-    CU_TRY(cudaMalloc(&b->d_cursor, 2 * sizeof(int32_t)));
-    CU_TRY(cudaMalloc(&b->d_cons, MP * (size_t)p.max_cons));
-    CU_TRY(cudaMalloc(&b->d_cov, MP * (size_t)p.max_cons * sizeof(uint16_t)));
-    CU_TRY(cudaMalloc(&b->d_len, MP * sizeof(int32_t)));
-    CU_TRY(cudaMalloc(&b->d_status, MP * sizeof(int32_t)));
-    CU_TRY(cudaMalloc(&b->d_out_off, MP * sizeof(int32_t)));
-    CU_TRY(cudaMalloc(&b->d_trim, MP * sizeof(int32_t)));
+        CU_TRY(cudaMemset(b->slab.p, std::atoi(env), (size_t)b->n_slots * b->slot_bytes));
+    CU_TRY(b->bases.alloc(AC));
+    CU_TRY(b->weights.alloc(AC));
+    CU_TRY(b->seq_off.alloc(MS + 1));
+    CU_TRY(b->w_off.alloc(MS + 1));
+    CU_TRY(b->seq_len.alloc(MS + 1));
+    CU_TRY(b->seq_begin.alloc(MS + 1));
+    CU_TRY(b->seq_end.alloc(MS + 1));
+    CU_TRY(b->win_seq_off.alloc(MP + 1));
+    CU_TRY(b->win_flags.alloc(MP));
+    CU_TRY(b->win_trim_nseq.alloc(MP));
+    CU_TRY(b->work.alloc(MP));
+    CU_TRY(b->cursor.alloc(2));
+    CU_TRY(b->cons.alloc(MP * (size_t)p.max_cons));
+    CU_TRY(b->cov.alloc(MP * (size_t)p.max_cons));
+    CU_TRY(b->len.alloc(MP));
+    CU_TRY(b->status.alloc(MP));
+    CU_TRY(b->out_off.alloc(MP));
+    CU_TRY(b->trim.alloc(MP));
     if (std::getenv("B200POA_PHASE_TIMERS")) {
-        CU_TRY(cudaMalloc(&b->d_phase, PH_COUNT * sizeof(unsigned long long)));
-        CU_TRY(cudaMemset(b->d_phase, 0, PH_COUNT * sizeof(unsigned long long)));
+        CU_TRY(b->phase.need(PH_COUNT * sizeof(unsigned long long), false));
+        CU_TRY(cudaMemset(b->phase.p, 0, PH_COUNT * sizeof(unsigned long long)));
     }
+    /* an estimate: of the per-sequence and per-window tables it counts 8 of 28 B a sequence and 16 of 32 B a window */
     b->device_bytes = (size_t)b->n_slots * b->slot_bytes + 2 * AC + (MS + 1) * 8 + MP * (16 + 3 * (size_t)p.max_cons);
     if (b->output_mask & B200POA_OUTPUT_MSA) {
-        CU_TRY(cudaMalloc(&b->d_path, AC * sizeof(uint16_t)));
-        CU_TRY(cudaMalloc(&b->d_msa, b->msa_cap));
-        CU_TRY(cudaMalloc(&b->d_msa_cursor, sizeof(unsigned long long)));
-        CU_TRY(cudaMalloc(&b->d_msa_off, MP * sizeof(long long)));
-        CU_TRY(cudaMalloc(&b->d_msa_cols, MP * sizeof(int32_t)));
-        CU_TRY(cudaMalloc(&b->d_msa_status, MP * sizeof(int32_t)));
-        CU_TRY(cudaHostAlloc(&b->h_msa_cursor, sizeof(unsigned long long), cudaHostAllocDefault));
-        CU_TRY(cudaHostAlloc(&b->h_msa_off, MP * sizeof(long long), cudaHostAllocDefault));
-        CU_TRY(cudaHostAlloc(&b->h_msa_cols, MP * sizeof(int32_t), cudaHostAllocDefault));
-        CU_TRY(cudaHostAlloc(&b->h_msa_status, MP * sizeof(int32_t), cudaHostAllocDefault));
-        CU_TRY(cudaHostAlloc(&b->h_msa_rows, MP * sizeof(int32_t), cudaHostAllocDefault));
+        CU_TRY(b->path.need(AC * sizeof(uint16_t), false));
+        CU_TRY(b->msa.need(b->msa_cap, false));
+        CU_TRY(b->msa_cursor.alloc(1));
+        CU_TRY(b->msa_off.alloc(MP));
+        CU_TRY(b->msa_cols.alloc(MP));
+        CU_TRY(b->msa_status.alloc(MP));
+        if (!b->h_msa_rows.reserve(MP * sizeof(int32_t))) return B200POA_CUDA_ERROR;
         b->device_bytes += AC * sizeof(uint16_t) + b->msa_cap + MP * 16;
     }
-    CU_TRY(cudaHostAlloc(&b->h_bases, AC, cudaHostAllocDefault));
-    CU_TRY(cudaHostAlloc(&b->h_weights, AC, cudaHostAllocDefault));
-    CU_TRY(cudaHostAlloc(&b->h_seq_off, (MS + 1) * sizeof(int64_t), cudaHostAllocDefault));
-    CU_TRY(cudaHostAlloc(&b->h_w_off, (MS + 1) * sizeof(int64_t), cudaHostAllocDefault));
-    CU_TRY(cudaHostAlloc(&b->h_seq_len, (MS + 1) * sizeof(int32_t), cudaHostAllocDefault));
-    CU_TRY(cudaHostAlloc(&b->h_seq_begin, (MS + 1) * sizeof(int32_t), cudaHostAllocDefault));
-    CU_TRY(cudaHostAlloc(&b->h_seq_end, (MS + 1) * sizeof(int32_t), cudaHostAllocDefault));
-    CU_TRY(cudaHostAlloc(&b->h_win_seq_off, (MP + 1) * sizeof(int32_t), cudaHostAllocDefault));
-    CU_TRY(cudaHostAlloc(&b->h_win_flags, MP * sizeof(int32_t), cudaHostAllocDefault));
-    CU_TRY(cudaHostAlloc(&b->h_win_trim_nseq, MP * sizeof(int32_t), cudaHostAllocDefault));
-    CU_TRY(cudaHostAlloc(&b->h_work, MP * sizeof(int32_t), cudaHostAllocDefault));
-    CU_TRY(cudaHostAlloc(&b->h_cons, MP * (size_t)p.max_cons, cudaHostAllocDefault));
-    CU_TRY(cudaHostAlloc(&b->h_cov, MP * (size_t)p.max_cons * sizeof(uint16_t), cudaHostAllocDefault));
-    CU_TRY(cudaHostAlloc(&b->h_len, MP * sizeof(int32_t), cudaHostAllocDefault));
-    CU_TRY(cudaHostAlloc(&b->h_status, MP * sizeof(int32_t), cudaHostAllocDefault));
-    CU_TRY(cudaHostAlloc(&b->h_out_off, MP * sizeof(int32_t), cudaHostAllocDefault));
-    CU_TRY(cudaHostAlloc(&b->h_trim, MP * sizeof(int32_t), cudaHostAllocDefault));
-    CU_TRY(cudaHostAlloc(&b->h_cursor, 2 * sizeof(int32_t), cudaHostAllocDefault));
 #if POA_FILL_DIGEST
-    CU_TRY(cudaMalloc(&b->d_fill_digest, (MS + 1) * sizeof(unsigned long long)));
-    CU_TRY(cudaMalloc(&b->d_fill_count, (MS + 1) * sizeof(int32_t)));
+    CU_TRY(b->fill_digest.need((MS + 1) * sizeof(unsigned long long), false));
+    CU_TRY(b->fill_count.need((MS + 1) * sizeof(int32_t), false));
 #endif
 #if POA_ALN_DIGEST
-    CU_TRY(cudaMalloc(&b->d_aln_digest, (MS + 1) * sizeof(unsigned long long)));
-    CU_TRY(cudaMalloc(&b->d_aln_count, (MS + 1) * sizeof(int32_t)));
+    CU_TRY(b->aln_digest.need((MS + 1) * sizeof(unsigned long long), false));
+    CU_TRY(b->aln_count.need((MS + 1) * sizeof(int32_t), false));
 #endif
 #if POA_GRAPH_DIGEST
-    CU_TRY(cudaMalloc(&b->d_graph_digest, (MS + 1) * sizeof(unsigned long long)));
-    CU_TRY(cudaMalloc(&b->d_graph_nodes, (MS + 1) * sizeof(int32_t)));
-    CU_TRY(cudaMalloc(&b->d_graph_edges, (MS + 1) * sizeof(int32_t)));
-    CU_TRY(cudaMalloc(&b->d_sub_digest, (MS + 1) * sizeof(unsigned long long)));
-    CU_TRY(cudaMalloc(&b->d_sub_count, (MS + 1) * sizeof(int32_t)));
-    CU_TRY(cudaMalloc(&b->d_cons_digest, 2 * (MP + 1) * sizeof(unsigned long long)));
-    CU_TRY(cudaMalloc(&b->d_cons_rounds, (MP + 1) * sizeof(int32_t)));
+    CU_TRY(b->graph_digest.need((MS + 1) * sizeof(unsigned long long), false));
+    CU_TRY(b->graph_nodes.need((MS + 1) * sizeof(int32_t), false));
+    CU_TRY(b->graph_edges.need((MS + 1) * sizeof(int32_t), false));
+    CU_TRY(b->sub_digest.need((MS + 1) * sizeof(unsigned long long), false));
+    CU_TRY(b->sub_count.need((MS + 1) * sizeof(int32_t), false));
+    CU_TRY(b->cons_digest.need(2 * (MP + 1) * sizeof(unsigned long long), false));
+    CU_TRY(b->cons_rounds.need((MP + 1) * sizeof(int32_t), false));
 #endif
     return B200POA_SUCCESS;
 }
@@ -760,14 +617,14 @@ int32_t b200poa_batch_create(int32_t device_id, void* stream, size_t max_gpu_mem
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || device_id < 0 || device_id >= ndev) return B200POA_CUDA_ERROR;
 
-    b200poa_batch* b = new (std::nothrow) b200poa_batch();
+    DeviceGuard guard(device_id);
+    std::unique_ptr<b200poa_batch> b(new (std::nothrow) b200poa_batch()); /* freed on every early return */
     if (!b) return B200POA_GENERIC_ERROR;
     b->id = g_batches++;
     b->device = device_id;
     b->stream = static_cast<cudaStream_t>(stream);
     b->output_mask = output_mask;
     b->cfg = *cfg;
-    DeviceGuard guard(device_id);
 
     Params& p = b->p;
     p.max_nodes = cfg->max_nodes_per_graph;
@@ -789,18 +646,12 @@ int32_t b200poa_batch_create(int32_t device_id, void* stream, size_t max_gpu_mem
     p.wide_cells = (p.force_cells32 || !score_range_ok(p, p.max_nodes, p.max_len)) ? 1 : 0;
     p.ring_rows = 8;
     p.ring_stride = p.stride;
-    if (p.max_nodes > 65000) {
-        delete b;
-        return B200POA_INVALID_ARGUMENT;
-    }
+    if (p.max_nodes > 65000) return B200POA_INVALID_ARGUMENT;
 
     Slot probe;
     slot_bind(probe, nullptr, p, &b->slot_bytes);
     cudaDeviceProp prop;
-    if (cudaGetDeviceProperties(&prop, device_id) != cudaSuccess) {
-        delete b;
-        return B200POA_CUDA_ERROR;
-    }
+    if (cudaGetDeviceProperties(&prop, device_id) != cudaSuccess) return B200POA_CUDA_ERROR;
     b->sm_count = prop.multiProcessorCount;
     /* worst-case shared memory (longest admissible read) must be launchable; the attribute is per function and per
      * device, so it is raised to the device's opt-in limit once and never lowered by a later, smaller batch */
@@ -808,28 +659,18 @@ int32_t b200poa_batch_create(int32_t device_id, void* stream, size_t max_gpu_mem
     if (worst.smem_bytes > (int32_t)prop.sharedMemPerBlockOptin) {
         std::fprintf(stderr, "[b200poa] batch %d: max_sequence_size %d needs %d B of shared memory per block (device limit %zu)\n",
                      b->id, p.max_len, worst.smem_bytes, (size_t)prop.sharedMemPerBlockOptin);
-        delete b;
         return B200POA_INVALID_ARGUMENT;
     }
     if (cudaFuncSetAttribute(poa_window_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             (int)prop.sharedMemPerBlockOptin) != cudaSuccess) {
-        delete b;
-        return B200POA_CUDA_ERROR;
-    }
+                             (int)prop.sharedMemPerBlockOptin) != cudaSuccess) return B200POA_CUDA_ERROR;
     /* slots are sized for the best occupancy a launch can reach (short reads => small profile) */
     int blocks_per_sm = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, poa_window_kernel, 32, 4096) != cudaSuccess) {
-        delete b;
-        return B200POA_CUDA_ERROR;
-    }
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, poa_window_kernel, 32, 4096) != cudaSuccess) return B200POA_CUDA_ERROR;
     if (const char* env = std::getenv("B200POA_BLOCKS_PER_SM")) {
         int v = std::atoi(env);
         if (v > 0 && v < blocks_per_sm) blocks_per_sm = v;
     }
-    if (blocks_per_sm < 1) {
-        delete b;
-        return B200POA_INVALID_ARGUMENT;
-    }
+    if (blocks_per_sm < 1) return B200POA_INVALID_ARGUMENT;
     b->blocks_per_sm = blocks_per_sm;
     int64_t want_slots = (int64_t)blocks_per_sm * prop.multiProcessorCount;
 
@@ -838,7 +679,6 @@ int32_t b200poa_batch_create(int32_t device_id, void* stream, size_t max_gpu_mem
     if (slots_by_mem < 1) {
         std::fprintf(stderr, "[b200poa] batch %d: %.2f GB is not enough for one window workspace (%.2f MB)\n",
                      b->id, max_gpu_mem / 1073741824.0, b->slot_bytes / 1048576.0);
-        delete b;
         return B200POA_INVALID_ARGUMENT;
     }
     b->n_slots = (int32_t)std::min(want_slots, slots_by_mem);
@@ -850,10 +690,7 @@ int32_t b200poa_batch_create(int32_t device_id, void* stream, size_t max_gpu_mem
         if (const char* env = std::getenv("B200POA_MSA_ARENA_MB")) cap_msa = (size_t)std::atoll(env) << 20;
         const size_t one = ((size_t)cfg->max_sequences_per_poa * (size_t)cfg->max_consensus_size + 15) & ~(size_t)15;
         if (cap_msa < one) cap_msa = one;
-        if (cap_msa >= rest) {
-            delete b;
-            return B200POA_INVALID_ARGUMENT;
-        }
+        if (cap_msa >= rest) return B200POA_INVALID_ARGUMENT;
         b->msa_cap = cap_msa;
         rest -= cap_msa;
     }
@@ -873,17 +710,12 @@ int32_t b200poa_batch_create(int32_t device_id, void* stream, size_t max_gpu_mem
     b->arena_cap = (int64_t)arena;
     b->max_seqs = std::max<int64_t>((int64_t)(arena / 10 / 8), 1024) + max_poas;
 
-    {
-        const int32_t ast = alloc_batch_memory(b);
-        if (ast != B200POA_SUCCESS) {
-            free_batch(b);
-            return ast;
-        }
-    }
-    b->h_seq_off[0] = 0;
-    b->h_win_seq_off[0] = 0;
+    const int32_t ast = alloc_batch_memory(b.get());
+    if (ast != B200POA_SUCCESS) return ast;
+    b->seq_off.h()[0] = 0;
+    b->win_seq_off.h()[0] = 0;
     b->cost.reserve((size_t)b->max_poas);
-    *out = b;
+    *out = b.release();
     return B200POA_SUCCESS;
 }
 
@@ -945,30 +777,30 @@ int32_t b200poa_batch_upload(b200poa_batch* b) {
     if (b->poa_count == 0) return B200POA_SUCCESS;
     DeviceGuard g(b->device);
     /* longest-first work list */
-    std::iota(b->h_work, b->h_work + b->poa_count, 0);
-    std::stable_sort(b->h_work, b->h_work + b->poa_count,
+    std::iota(b->work.h(), b->work.h() + b->poa_count, 0);
+    std::stable_sort(b->work.h(), b->work.h() + b->poa_count,
                      [&](int32_t x, int32_t y) { return b->cost[(size_t)x] > b->cost[(size_t)y]; });
     const size_t W = (size_t)b->poa_count, S = (size_t)b->seq_count;
     int64_t weight_bytes = b->weight_count;
     if (b->ext_bases) { /* direct mode: the caller's pinned arena range goes up as it is */
-        CU_TRY(cudaMemcpyAsync(b->d_bases, b->ext_bases + b->ext_lo, (size_t)b->base_count, cudaMemcpyHostToDevice, b->stream));
+        CU_TRY(cudaMemcpyAsync(b->bases.d(), b->ext_bases + b->ext_lo, (size_t)b->base_count, cudaMemcpyHostToDevice, b->stream));
         weight_bytes = b->ext_any_weights ? b->base_count : 0;
         if (weight_bytes > 0)
-            CU_TRY(cudaMemcpyAsync(b->d_weights, b->ext_weights + b->ext_lo, (size_t)weight_bytes, cudaMemcpyHostToDevice, b->stream));
+            CU_TRY(cudaMemcpyAsync(b->weights.d(), b->ext_weights + b->ext_lo, (size_t)weight_bytes, cudaMemcpyHostToDevice, b->stream));
     } else {
-        CU_TRY(cudaMemcpyAsync(b->d_bases, b->h_bases, (size_t)b->base_count, cudaMemcpyHostToDevice, b->stream));
+        CU_TRY(b->bases.upload((size_t)b->base_count, b->stream));
         if (weight_bytes > 0) /* only sequences with non-constant weights carry bytes */
-            CU_TRY(cudaMemcpyAsync(b->d_weights, b->h_weights, (size_t)weight_bytes, cudaMemcpyHostToDevice, b->stream));
+            CU_TRY(b->weights.upload((size_t)weight_bytes, b->stream));
     }
-    CU_TRY(cudaMemcpyAsync(b->d_seq_off, b->h_seq_off, S * sizeof(int64_t), cudaMemcpyHostToDevice, b->stream));
-    CU_TRY(cudaMemcpyAsync(b->d_seq_len, b->h_seq_len, S * sizeof(int32_t), cudaMemcpyHostToDevice, b->stream));
-    CU_TRY(cudaMemcpyAsync(b->d_w_off, b->h_w_off, S * sizeof(int64_t), cudaMemcpyHostToDevice, b->stream));
-    CU_TRY(cudaMemcpyAsync(b->d_seq_begin, b->h_seq_begin, S * sizeof(int32_t), cudaMemcpyHostToDevice, b->stream));
-    CU_TRY(cudaMemcpyAsync(b->d_seq_end, b->h_seq_end, S * sizeof(int32_t), cudaMemcpyHostToDevice, b->stream));
-    CU_TRY(cudaMemcpyAsync(b->d_win_seq_off, b->h_win_seq_off, (W + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, b->stream));
-    CU_TRY(cudaMemcpyAsync(b->d_win_flags, b->h_win_flags, W * sizeof(int32_t), cudaMemcpyHostToDevice, b->stream));
-    CU_TRY(cudaMemcpyAsync(b->d_win_trim_nseq, b->h_win_trim_nseq, W * sizeof(int32_t), cudaMemcpyHostToDevice, b->stream));
-    CU_TRY(cudaMemcpyAsync(b->d_work, b->h_work, W * sizeof(int32_t), cudaMemcpyHostToDevice, b->stream));
+    CU_TRY(b->seq_off.upload(S, b->stream));
+    CU_TRY(b->seq_len.upload(S, b->stream));
+    CU_TRY(b->w_off.upload(S, b->stream));
+    CU_TRY(b->seq_begin.upload(S, b->stream));
+    CU_TRY(b->seq_end.upload(S, b->stream));
+    CU_TRY(b->win_seq_off.upload(W + 1, b->stream));
+    CU_TRY(b->win_flags.upload(W, b->stream));
+    CU_TRY(b->win_trim_nseq.upload(W, b->stream));
+    CU_TRY(b->work.upload(W, b->stream));
     b->h2d_bytes = b->base_count + weight_bytes + (int64_t)(S * 28 + (W + 1) * 4 + W * 12);
     b->uploaded = true;
     return B200POA_SUCCESS;
@@ -979,38 +811,38 @@ int32_t b200poa_batch_launch(b200poa_batch* b) {
     if (b->poa_count == 0) return B200POA_SUCCESS;
     if (!b->uploaded) return B200POA_INVALID_ARGUMENT;
     DeviceGuard g(b->device);
-    CU_TRY(cudaMemsetAsync(b->d_cursor, 0, 2 * sizeof(int32_t), b->stream));
-    if (b->d_msa_cursor) CU_TRY(cudaMemsetAsync(b->d_msa_cursor, 0, sizeof(unsigned long long), b->stream));
+    CU_TRY(cudaMemsetAsync(b->cursor.d(), 0, 2 * sizeof(int32_t), b->stream));
+    if (b->msa_cursor.d()) CU_TRY(cudaMemsetAsync(b->msa_cursor.d(), 0, sizeof(unsigned long long), b->stream));
     KernelArgs a;
     a.p = b->p;
-    a.slab = b->d_slab;
+    a.slab = static_cast<uint8_t*>(b->slab.p);
     a.slot_bytes = b->slot_bytes;
     a.n_windows = b->poa_count;
-    a.work = b->d_work;
-    a.cursor = b->d_cursor;
-    a.bases = b->d_bases;
-    a.weights = b->d_weights;
-    a.seq_off = b->d_seq_off;
-    a.seq_len = b->d_seq_len;
-    a.w_off = b->d_w_off;
-    a.win_seq_off = b->d_win_seq_off;
-    a.win_flags = b->d_win_flags;
-    a.win_trim_nseq = b->d_win_trim_nseq;
-    a.seq_begin = b->d_seq_begin;
-    a.seq_end = b->d_seq_end;
-    a.out_cons = b->d_cons;
-    a.out_cov = b->d_cov;
-    a.out_len = b->d_len;
-    a.out_status = b->d_status;
-    a.out_off = b->d_out_off;
-    a.out_trim = b->d_trim;
-    a.path = b->d_path;
-    a.out_msa = b->d_msa;
-    a.msa_cursor = b->d_msa_cursor;
+    a.work = b->work.d();
+    a.cursor = b->cursor.d();
+    a.bases = b->bases.d();
+    a.weights = b->weights.d();
+    a.seq_off = b->seq_off.d();
+    a.seq_len = b->seq_len.d();
+    a.w_off = b->w_off.d();
+    a.win_seq_off = b->win_seq_off.d();
+    a.win_flags = b->win_flags.d();
+    a.win_trim_nseq = b->win_trim_nseq.d();
+    a.seq_begin = b->seq_begin.d();
+    a.seq_end = b->seq_end.d();
+    a.out_cons = b->cons.d();
+    a.out_cov = b->cov.d();
+    a.out_len = b->len.d();
+    a.out_status = b->status.d();
+    a.out_off = b->out_off.d();
+    a.out_trim = b->trim.d();
+    a.path = static_cast<uint16_t*>(b->path.p);
+    a.out_msa = static_cast<uint8_t*>(b->msa.p);
+    a.msa_cursor = b->msa_cursor.d();
     a.msa_cap = (unsigned long long)b->msa_cap;
-    a.out_msa_off = b->d_msa_off;
-    a.out_msa_cols = b->d_msa_cols;
-    a.out_msa_status = b->d_msa_status;
+    a.out_msa_off = b->msa_off.d();
+    a.out_msa_cols = b->msa_cols.d();
+    a.out_msa_status = b->msa_status.d();
     a.p.skip_consensus = (b->output_mask & B200POA_OUTPUT_CONSENSUS) ? 0 : 1;
     /* shared memory geometry follows the longest read actually staged */
     const SmemGeometry sg = smem_geometry(b->p, b->max_len_staged);
@@ -1027,37 +859,37 @@ int32_t b200poa_batch_launch(b200poa_batch* b) {
     a.ring_rows = b->ring_rows;
     a.p.ring_rows = b->ring_rows;
     a.p.ring_stride = b->ring_stride;
-    a.phase_cycles = b->d_phase;
+    a.phase_cycles = static_cast<unsigned long long*>(b->phase.p);
 #if POA_FILL_DIGEST
-    CU_TRY(cudaMemsetAsync(b->d_fill_digest, 0, (size_t)b->seq_count * sizeof(unsigned long long), b->stream));
-    CU_TRY(cudaMemsetAsync(b->d_fill_count, 0, (size_t)b->seq_count * sizeof(int32_t), b->stream));
-    a.fill_digest = b->d_fill_digest;
-    a.fill_count = b->d_fill_count;
+    CU_TRY(cudaMemsetAsync(b->fill_digest.p, 0, (size_t)b->seq_count * sizeof(unsigned long long), b->stream));
+    CU_TRY(cudaMemsetAsync(b->fill_count.p, 0, (size_t)b->seq_count * sizeof(int32_t), b->stream));
+    a.fill_digest = static_cast<unsigned long long*>(b->fill_digest.p);
+    a.fill_count = static_cast<int32_t*>(b->fill_count.p);
 #endif
 #if POA_ALN_DIGEST
-    CU_TRY(cudaMemsetAsync(b->d_aln_digest, 0, (size_t)b->seq_count * sizeof(unsigned long long), b->stream));
-    CU_TRY(cudaMemsetAsync(b->d_aln_count, 0, (size_t)b->seq_count * sizeof(int32_t), b->stream));
-    a.aln_digest = b->d_aln_digest;
-    a.aln_count = b->d_aln_count;
+    CU_TRY(cudaMemsetAsync(b->aln_digest.p, 0, (size_t)b->seq_count * sizeof(unsigned long long), b->stream));
+    CU_TRY(cudaMemsetAsync(b->aln_count.p, 0, (size_t)b->seq_count * sizeof(int32_t), b->stream));
+    a.aln_digest = static_cast<unsigned long long*>(b->aln_digest.p);
+    a.aln_count = static_cast<int32_t*>(b->aln_count.p);
 #endif
 #if POA_GRAPH_DIGEST
     {
         const size_t ns = (size_t)b->seq_count, nw = (size_t)b->poa_count;
-        CU_TRY(cudaMemsetAsync(b->d_graph_digest, 0, ns * sizeof(unsigned long long), b->stream));
-        CU_TRY(cudaMemsetAsync(b->d_graph_nodes, 0, ns * sizeof(int32_t), b->stream));
-        CU_TRY(cudaMemsetAsync(b->d_graph_edges, 0, ns * sizeof(int32_t), b->stream));
-        CU_TRY(cudaMemsetAsync(b->d_sub_digest, 0, ns * sizeof(unsigned long long), b->stream));
-        CU_TRY(cudaMemsetAsync(b->d_sub_count, 0, ns * sizeof(int32_t), b->stream));
-        CU_TRY(cudaMemsetAsync(b->d_cons_digest, 0, 2 * nw * sizeof(unsigned long long), b->stream));
-        CU_TRY(cudaMemsetAsync(b->d_cons_rounds, 0, nw * sizeof(int32_t), b->stream));
+        CU_TRY(cudaMemsetAsync(b->graph_digest.p, 0, ns * sizeof(unsigned long long), b->stream));
+        CU_TRY(cudaMemsetAsync(b->graph_nodes.p, 0, ns * sizeof(int32_t), b->stream));
+        CU_TRY(cudaMemsetAsync(b->graph_edges.p, 0, ns * sizeof(int32_t), b->stream));
+        CU_TRY(cudaMemsetAsync(b->sub_digest.p, 0, ns * sizeof(unsigned long long), b->stream));
+        CU_TRY(cudaMemsetAsync(b->sub_count.p, 0, ns * sizeof(int32_t), b->stream));
+        CU_TRY(cudaMemsetAsync(b->cons_digest.p, 0, 2 * nw * sizeof(unsigned long long), b->stream));
+        CU_TRY(cudaMemsetAsync(b->cons_rounds.p, 0, nw * sizeof(int32_t), b->stream));
     }
-    a.graph_digest = b->d_graph_digest;
-    a.graph_nodes = b->d_graph_nodes;
-    a.graph_edges = b->d_graph_edges;
-    a.sub_digest = b->d_sub_digest;
-    a.sub_count = b->d_sub_count;
-    a.cons_digest = b->d_cons_digest;
-    a.cons_rounds = b->d_cons_rounds;
+    a.graph_digest = static_cast<unsigned long long*>(b->graph_digest.p);
+    a.graph_nodes = static_cast<int32_t*>(b->graph_nodes.p);
+    a.graph_edges = static_cast<int32_t*>(b->graph_edges.p);
+    a.sub_digest = static_cast<unsigned long long*>(b->sub_digest.p);
+    a.sub_count = static_cast<int32_t*>(b->sub_count.p);
+    a.cons_digest = static_cast<unsigned long long*>(b->cons_digest.p);
+    a.cons_rounds = static_cast<int32_t*>(b->cons_rounds.p);
 #endif
     /* persistent grid: one warp per resident slot */
     const int grid = std::max(1, std::min(std::min(b->n_slots, occ * b->sm_count), b->poa_count));
@@ -1078,16 +910,16 @@ int32_t b200poa_batch_download(b200poa_batch* b) {
     if (b->poa_count == 0) return B200POA_SUCCESS;
     DeviceGuard g(b->device);
     const size_t W = (size_t)b->poa_count;
-    CU_TRY(cudaMemcpyAsync(b->h_len, b->d_len, W * sizeof(int32_t), cudaMemcpyDeviceToHost, b->stream));
-    CU_TRY(cudaMemcpyAsync(b->h_status, b->d_status, W * sizeof(int32_t), cudaMemcpyDeviceToHost, b->stream));
-    CU_TRY(cudaMemcpyAsync(b->h_out_off, b->d_out_off, W * sizeof(int32_t), cudaMemcpyDeviceToHost, b->stream));
-    CU_TRY(cudaMemcpyAsync(b->h_trim, b->d_trim, W * sizeof(int32_t), cudaMemcpyDeviceToHost, b->stream));
-    CU_TRY(cudaMemcpyAsync(b->h_cursor, b->d_cursor, 2 * sizeof(int32_t), cudaMemcpyDeviceToHost, b->stream));
-    if (b->d_msa) { /* the MSA tables; the rows follow in b200poa_batch_get_msa once the fill level is known */
-        CU_TRY(cudaMemcpyAsync(b->h_msa_off, b->d_msa_off, W * sizeof(long long), cudaMemcpyDeviceToHost, b->stream));
-        CU_TRY(cudaMemcpyAsync(b->h_msa_cols, b->d_msa_cols, W * sizeof(int32_t), cudaMemcpyDeviceToHost, b->stream));
-        CU_TRY(cudaMemcpyAsync(b->h_msa_status, b->d_msa_status, W * sizeof(int32_t), cudaMemcpyDeviceToHost, b->stream));
-        CU_TRY(cudaMemcpyAsync(b->h_msa_cursor, b->d_msa_cursor, sizeof(unsigned long long), cudaMemcpyDeviceToHost, b->stream));
+    CU_TRY(b->len.download(W, b->stream));
+    CU_TRY(b->status.download(W, b->stream));
+    CU_TRY(b->out_off.download(W, b->stream));
+    CU_TRY(b->trim.download(W, b->stream));
+    CU_TRY(b->cursor.download(2, b->stream));
+    if (b->msa.p) { /* the MSA tables; the rows follow in b200poa_batch_get_msa once the fill level is known */
+        CU_TRY(b->msa_off.download(W, b->stream));
+        CU_TRY(b->msa_cols.download(W, b->stream));
+        CU_TRY(b->msa_status.download(W, b->stream));
+        CU_TRY(b->msa_cursor.download(1, b->stream));
     }
     return B200POA_SUCCESS;
 }
@@ -1108,23 +940,22 @@ int32_t b200poa_batch_get_consensus(b200poa_batch* b, const uint8_t** cons, cons
     DeviceGuard g(b->device);
     CU_TRY(cudaStreamSynchronize(b->stream));
     if (b->poa_count > 0 && !b->results_fetched) { /* D2H, second half: the used part of the compact arenas */
-        const size_t used = (size_t)(uint32_t)b->h_cursor[1];
+        const size_t used = (size_t)(uint32_t)b->cursor.h()[1];
         b->out_elems = (int64_t)used;
         if (used > 0) {
-            CU_TRY(cudaMemcpyAsync(b->h_cons, b->d_cons, used, cudaMemcpyDeviceToHost, b->stream));
-            if (b->download_coverage)
-                CU_TRY(cudaMemcpyAsync(b->h_cov, b->d_cov, used * sizeof(uint16_t), cudaMemcpyDeviceToHost, b->stream));
+            CU_TRY(b->cons.download(used, b->stream));
+            if (b->download_coverage) CU_TRY(b->cov.download(used, b->stream));
             CU_TRY(cudaStreamSynchronize(b->stream));
         }
         b->d2h_bytes = (int64_t)b->poa_count * 16 + 8 + (int64_t)used * (b->download_coverage ? 3 : 1);
         b->results_fetched = true;
     }
-    if (cons) *cons = b->h_cons;
-    if (cov) *cov = b->download_coverage ? b->h_cov : nullptr;
-    if (lens) *lens = b->h_len;
-    if (status) *status = b->h_status;
-    if (offsets) *offsets = b->h_out_off;
-    if (trim) *trim = b->h_trim;
+    if (cons) *cons = b->cons.h();
+    if (cov) *cov = b->download_coverage ? b->cov.h() : nullptr;
+    if (lens) *lens = b->len.h();
+    if (status) *status = b->status.h();
+    if (offsets) *offsets = b->out_off.h();
+    if (trim) *trim = b->trim.h();
     return B200POA_SUCCESS;
 }
 
@@ -1136,27 +967,21 @@ int32_t b200poa_batch_get_msa(b200poa_batch* b, const uint8_t** msa, const int64
     CU_TRY(cudaStreamSynchronize(b->stream));
     if (b->poa_count > 0 && !b->msa_fetched) { /* exactly the bytes the launch used (the reference copies
                                                   max_poas x max_sequences_per_poa x max_consensus_size, :271-275) */
-        const size_t used = (size_t)*b->h_msa_cursor;
-        if (used > b->h_msa_bytes) {
-            cudaFreeHost(b->h_msa);
-            b->h_msa = nullptr;
-            b->h_msa_bytes = 0;
-            CU_TRY(cudaHostAlloc(&b->h_msa, used + used / 4, cudaHostAllocDefault));
-            b->h_msa_bytes = used + used / 4;
-        }
+        const size_t used = (size_t)*b->msa_cursor.h();
+        if (!b->h_msa.reserve(used)) return B200POA_CUDA_ERROR;
         if (used > 0) {
-            CU_TRY(cudaMemcpyAsync(b->h_msa, b->d_msa, used, cudaMemcpyDeviceToHost, b->stream));
+            CU_TRY(cudaMemcpyAsync(b->h_msa.p, b->msa.p, used, cudaMemcpyDeviceToHost, b->stream));
             CU_TRY(cudaStreamSynchronize(b->stream));
         }
         b->d2h_bytes += (int64_t)used + (int64_t)b->poa_count * 16 + 8;
         b->msa_fetched = true;
     }
     static_assert(sizeof(long long) == sizeof(int64_t), "offset table type");
-    if (msa) *msa = b->h_msa;
-    if (offsets) *offsets = reinterpret_cast<const int64_t*>(b->h_msa_off);
-    if (n_rows) *n_rows = b->h_msa_rows;
-    if (n_cols) *n_cols = b->h_msa_cols;
-    if (status) *status = b->h_msa_status;
+    if (msa) *msa = b->h_msa.p;
+    if (offsets) *offsets = reinterpret_cast<const int64_t*>(b->msa_off.h());
+    if (n_rows) *n_rows = reinterpret_cast<const int32_t*>(b->h_msa_rows.p);
+    if (n_cols) *n_cols = b->msa_cols.h();
+    if (status) *status = b->msa_status.h();
     return B200POA_SUCCESS;
 }
 
@@ -1191,15 +1016,19 @@ int32_t b200poa_batch_reset(b200poa_batch* b) {
     return B200POA_SUCCESS;
 }
 
-void b200poa_batch_destroy(b200poa_batch* b) { free_batch(b); }
+void b200poa_batch_destroy(b200poa_batch* b) {
+    if (!b) return;
+    DeviceGuard g(b->device);
+    delete b;
+}
 
 int32_t b200poa_batch_phase_cycles(b200poa_batch* b, uint64_t* out, int32_t n) {
     /* diagnostics (B200POA_PHASE_TIMERS=1): cycles per phase summed over warps since creation */
-    if (!b || !out || !b->d_phase) return B200POA_OUTPUT_TYPE_UNAVAILABLE;
+    if (!b || !out || !b->phase.p) return B200POA_OUTPUT_TYPE_UNAVAILABLE;
     unsigned long long h[PH_COUNT];
     DeviceGuard g(b->device);
     CU_TRY(cudaStreamSynchronize(b->stream));
-    CU_TRY(cudaMemcpy(h, b->d_phase, sizeof(h), cudaMemcpyDeviceToHost));
+    CU_TRY(cudaMemcpy(h, b->phase.p, sizeof(h), cudaMemcpyDeviceToHost));
     for (int32_t i = 0; i < n && i < PH_COUNT; ++i) out[i] = h[i];
     return B200POA_SUCCESS;
 }
@@ -1231,8 +1060,8 @@ extern "C" int32_t b200poa_debug_fill_digest(b200poa_batch* b, uint64_t* digest,
     if (!b || !digest || !count || n < b->seq_count) return B200POA_INVALID_ARGUMENT;
     DeviceGuard g(b->device);
     CU_TRY(cudaStreamSynchronize(b->stream));
-    CU_TRY(cudaMemcpy(digest, b->d_fill_digest, (size_t)b->seq_count * sizeof(uint64_t), cudaMemcpyDeviceToHost));
-    CU_TRY(cudaMemcpy(count, b->d_fill_count, (size_t)b->seq_count * sizeof(int32_t), cudaMemcpyDeviceToHost));
+    CU_TRY(cudaMemcpy(digest, b->fill_digest.p, (size_t)b->seq_count * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+    CU_TRY(cudaMemcpy(count, b->fill_count.p, (size_t)b->seq_count * sizeof(int32_t), cudaMemcpyDeviceToHost));
     if (ring_rows) *ring_rows = b->ring_rows;
     if (ring_stride) *ring_stride = b->ring_stride;
     return B200POA_SUCCESS;
@@ -1245,8 +1074,8 @@ extern "C" int32_t b200poa_debug_aln_digest(b200poa_batch* b, uint64_t* digest, 
     if (!b || !digest || !count || n < b->seq_count) return B200POA_INVALID_ARGUMENT;
     DeviceGuard g(b->device);
     CU_TRY(cudaStreamSynchronize(b->stream));
-    CU_TRY(cudaMemcpy(digest, b->d_aln_digest, (size_t)b->seq_count * sizeof(uint64_t), cudaMemcpyDeviceToHost));
-    CU_TRY(cudaMemcpy(count, b->d_aln_count, (size_t)b->seq_count * sizeof(int32_t), cudaMemcpyDeviceToHost));
+    CU_TRY(cudaMemcpy(digest, b->aln_digest.p, (size_t)b->seq_count * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+    CU_TRY(cudaMemcpy(count, b->aln_count.p, (size_t)b->seq_count * sizeof(int32_t), cudaMemcpyDeviceToHost));
     return B200POA_SUCCESS;
 }
 #endif
@@ -1265,13 +1094,13 @@ extern "C" int32_t b200poa_debug_graph_digest(b200poa_batch* b, uint64_t* graph_
     DeviceGuard g(b->device);
     CU_TRY(cudaStreamSynchronize(b->stream));
     const size_t ns = (size_t)b->seq_count, nw = (size_t)b->poa_count;
-    CU_TRY(cudaMemcpy(graph_digest, b->d_graph_digest, ns * sizeof(uint64_t), cudaMemcpyDeviceToHost));
-    CU_TRY(cudaMemcpy(graph_nodes, b->d_graph_nodes, ns * sizeof(int32_t), cudaMemcpyDeviceToHost));
-    CU_TRY(cudaMemcpy(graph_edges, b->d_graph_edges, ns * sizeof(int32_t), cudaMemcpyDeviceToHost));
-    CU_TRY(cudaMemcpy(sub_digest, b->d_sub_digest, ns * sizeof(uint64_t), cudaMemcpyDeviceToHost));
-    CU_TRY(cudaMemcpy(sub_count, b->d_sub_count, ns * sizeof(int32_t), cudaMemcpyDeviceToHost));
-    CU_TRY(cudaMemcpy(cons_digest, b->d_cons_digest, 2 * nw * sizeof(uint64_t), cudaMemcpyDeviceToHost));
-    CU_TRY(cudaMemcpy(cons_rounds, b->d_cons_rounds, nw * sizeof(int32_t), cudaMemcpyDeviceToHost));
+    CU_TRY(cudaMemcpy(graph_digest, b->graph_digest.p, ns * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+    CU_TRY(cudaMemcpy(graph_nodes, b->graph_nodes.p, ns * sizeof(int32_t), cudaMemcpyDeviceToHost));
+    CU_TRY(cudaMemcpy(graph_edges, b->graph_edges.p, ns * sizeof(int32_t), cudaMemcpyDeviceToHost));
+    CU_TRY(cudaMemcpy(sub_digest, b->sub_digest.p, ns * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+    CU_TRY(cudaMemcpy(sub_count, b->sub_count.p, ns * sizeof(int32_t), cudaMemcpyDeviceToHost));
+    CU_TRY(cudaMemcpy(cons_digest, b->cons_digest.p, 2 * nw * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+    CU_TRY(cudaMemcpy(cons_rounds, b->cons_rounds.p, nw * sizeof(int32_t), cudaMemcpyDeviceToHost));
     return B200POA_SUCCESS;
 }
 #endif

@@ -8,6 +8,8 @@
 #include <stdexcept>
 #include <string>
 
+#include "../cuda_buffers.hpp"
+
 namespace racon_b200 {
 
 using namespace b200poa_cpp;
@@ -25,30 +27,22 @@ CUDABatchProcessor::CUDABatchProcessor(uint32_t max_window_depth, uint32_t devic
                                        int8_t mismatch, int8_t match, bool cuda_banded_alignment, bool trim)
     : device_(device), trim_(trim) {
     bid_ = CUDABatchProcessor::batches++;
-    int prev = 0;
-    cudaGetDevice(&prev);
-    cudaSetDevice(static_cast<int>(device));
+    b200buf::DeviceGuard guard(static_cast<int>(device));
     cudaStream_t s = nullptr;
-    if (cudaStreamCreate(&s) != cudaSuccess) { /* cudabatch.cpp:54 */
-        cudaSetDevice(prev);
+    if (cudaStreamCreate(&s) != cudaSuccess) /* cudabatch.cpp:54 */
         throw std::runtime_error("[racon_b200::CUDABatchProcessor] cudaStreamCreate failed");
-    }
     stream_ = s;
     /* cudabatch.cpp:56-68 */
     BatchConfig batch_config(1023, static_cast<int32_t>(max_window_depth), 256,
                              cuda_banded_alignment ? BandMode::static_band : BandMode::full_band);
     cudapoa_batch_ = create_batch(static_cast<int32_t>(device), stream_, avail_mem, OutputType::consensus,
                                   batch_config, gap, mismatch, match);
-    cudaSetDevice(prev);
 }
 
 CUDABatchProcessor::~CUDABatchProcessor() {
     cudapoa_batch_.reset();
-    int prev = 0;
-    cudaGetDevice(&prev);
-    cudaSetDevice(static_cast<int>(device_));
+    b200buf::DeviceGuard guard(static_cast<int>(device_));
     cudaStreamDestroy(static_cast<cudaStream_t>(stream_)); /* cudabatch.cpp:74 */
-    cudaSetDevice(prev);
 }
 
 void CUDABatchProcessor::convertPhredQualityToWeights(const char* qual, uint32_t qual_length,

@@ -14,6 +14,7 @@
 #include <string>
 #include <thread>
 
+#include "../cuda_buffers.hpp"
 #include "b200poa.h"
 #include "cuda_batch.hpp"
 #include "window_arena.hpp"
@@ -35,11 +36,8 @@ static std::vector<int32_t> resolve_devices(const std::vector<int32_t>& want) {
 static size_t batch_memory(int32_t device, uint32_t batches, size_t requested) {
     if (requested) return requested;
     size_t free_b = 0, total = 0;
-    int prev = 0;
-    cudaGetDevice(&prev);
-    cudaSetDevice(device);
+    b200buf::DeviceGuard guard(device);
     cudaMemGetInfo(&free_b, &total);
-    cudaSetDevice(prev);
     return static_cast<size_t>(0.9 * static_cast<double>(free_b) / batches); /* cudapolisher.cpp:233-236 */
 }
 
