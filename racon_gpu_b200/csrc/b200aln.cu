@@ -421,28 +421,11 @@ __global__ void aln_cut_filter_kernel(const CutArgs a) {
  * scanned in shared memory, then each thread writes its chunk's offsets */
 __global__ void __launch_bounds__(1024) aln_cut_scan_kernel(const CutArgs a) {
     __shared__ int64_t part[1024];
-    const int64_t chunk = (a.n_win + 1023) / 1024;
-    const int64_t lo0 = (int64_t)threadIdx.x * chunk;
-    const int64_t lo = lo0 < a.n_win ? lo0 : a.n_win, hi = lo + chunk < a.n_win ? lo + chunk : a.n_win;
-    int64_t sum = 0;
-    for (int64_t i = lo; i < hi; ++i) sum += a.counts[i];
-    part[threadIdx.x] = sum;
+    cut_scan_sum(a, threadIdx.x, 1024, part);
     __syncthreads();
-    if (threadIdx.x == 0) {
-        int64_t run = 0;
-        for (int i = 0; i < 1024; ++i) {
-            const int64_t v = part[i];
-            part[i] = run;
-            run += v;
-        }
-        a.win_off[a.n_win] = run;
-    }
+    if (threadIdx.x == 0) cut_scan_parts(a, 1024, part);
     __syncthreads();
-    int64_t run = part[threadIdx.x];
-    for (int64_t i = lo; i < hi; ++i) {
-        a.win_off[i] = run;
-        run += a.counts[i];
-    }
+    cut_scan_write(a, threadIdx.x, 1024, part);
 }
 __global__ void aln_cut_scatter_kernel(const CutArgs a) {
     for (int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; p < a.n_items; p += (int64_t)gridDim.x * blockDim.x)

@@ -114,6 +114,37 @@ CUT_FN void cut_filter(const CutArgs& a, int64_t p) {
     a.items[p] = r;
 }
 
+/* phase 2: exclusive prefix sum of the per-window counts in one block of nt threads, in three steps with a barrier
+ * between them.  Each thread sums a contiguous chunk of ceil(n_win / nt) windows into part[t]; thread 0 scans the
+ * chunk sums and writes the total to win_off[n_win]; then each thread writes its chunk's offsets. */
+CUT_FN void cut_scan_sum(const CutArgs& a, uint32_t t, uint32_t nt, int64_t* part) {
+    const int64_t chunk = (a.n_win + (nt - 1)) / nt;
+    const int64_t lo0 = (int64_t)t * chunk;
+    const int64_t lo = lo0 < a.n_win ? lo0 : a.n_win, hi = lo + chunk < a.n_win ? lo + chunk : a.n_win;
+    int64_t sum = 0;
+    for (int64_t i = lo; i < hi; ++i) sum += a.counts[i];
+    part[t] = sum;
+}
+CUT_FN void cut_scan_parts(const CutArgs& a, uint32_t nt, int64_t* part) {
+    int64_t run = 0;
+    for (int i = 0; i < (int)nt; ++i) {
+        const int64_t v = part[i];
+        part[i] = run;
+        run += v;
+    }
+    a.win_off[a.n_win] = run;
+}
+CUT_FN void cut_scan_write(const CutArgs& a, uint32_t t, uint32_t nt, const int64_t* part) {
+    const int64_t chunk = (a.n_win + (nt - 1)) / nt;
+    const int64_t lo0 = (int64_t)t * chunk;
+    const int64_t lo = lo0 < a.n_win ? lo0 : a.n_win, hi = lo + chunk < a.n_win ? lo + chunk : a.n_win;
+    int64_t run = part[t];
+    for (int64_t i = lo; i < hi; ++i) {
+        a.win_off[i] = run;
+        run += a.counts[i];
+    }
+}
+
 /* phase 3 for item p */
 CUT_FN void cut_scatter(const CutArgs& a, int64_t p) {
     const int32_t win = a.items[p].window;

@@ -1,7 +1,8 @@
 /*
  * emu_cut.cpp -- host build of the device layer cut (racon_gpu_b200/csrc/layer_cut.cuh; TEST INFRASTRUCTURE).
  *
- * Runs the four phases exactly as b200aln.cu launches them, one loop per launch; phase 3 (the scatter, whose order on
+ * Runs the four phases exactly as b200aln.cu launches them, one loop per launch; phase 2 (the scan) runs its three
+ * steps for 1024 emulated threads, as the one block of aln_cut_scan_kernel does; phase 3 (the scatter, whose order on
  * the device is whatever the atomics make it) visits the items in a seeded random order, so the tests see that the
  * final grouping does not depend on it.  Never linked into the product library.
  */
@@ -18,6 +19,24 @@ using namespace b200aln;
 extern "C" {
 
 int32_t emu_cut_layer_bytes(void) { return (int32_t)sizeof(CutLayer); }
+
+/* phase 2 as aln_cut_scan_kernel runs it: one block of 1024 threads, a barrier between the steps */
+static void run_scan(const CutArgs& a) {
+    const uint32_t nt = 1024;
+    std::vector<int64_t> part(nt);
+    for (uint32_t t = 0; t < nt; ++t) cut_scan_sum(a, t, nt, part.data());
+    cut_scan_parts(a, nt, part.data());
+    for (uint32_t t = 0; t < nt; ++t) cut_scan_write(a, t, nt, part.data());
+}
+
+/* phase 2 alone: win_off[n_win + 1] from counts[n_win] */
+void emu_cut_scan(const int32_t* counts, int64_t n_win, int64_t* win_off) {
+    CutArgs a{};
+    a.counts = const_cast<int32_t*>(counts);
+    a.n_win = n_win;
+    a.win_off = win_off;
+    run_scan(a);
+}
 
 /* n overlaps: q_off into `qual`'s arena, bp_off (pairs) into bp, bp_count (pairs), first_window, q_first, has_quality.
  * Writes up to the number of items records to out and n_win counts; returns the number of kept layers. */
@@ -52,7 +71,7 @@ int64_t emu_layer_cut(int32_t n, const int64_t* q_off, const int64_t* bp_off, co
     a.slots = slots.data();
     a.out = out;
     for (int64_t p = 0; p < n_items; ++p) cut_filter(a, p);
-    for (int64_t w = 0; w < n_win; ++w) win_off[(size_t)w + 1] = win_off[(size_t)w] + counts[w];
+    run_scan(a);
     std::vector<int64_t> order((size_t)n_items);
     std::iota(order.begin(), order.end(), 0);
     std::mt19937_64 rng(seed);

@@ -2,9 +2,11 @@
 
 `synth_overlap_set` makes contigs, reads drawn from them with errors (either strand, with or without qualities) and the
 overlaps racon would keep, in racon's order; `host_path` polishes them the way racon does without the device cut:
-breaking points from the aligner, the loop of src/polisher.cpp:384-457 on the host into a window arena, then
-b200poa_polisher_polish_arena."""
+breaking points from the aligner, the loop of src/polisher.cpp:384-457 (cut_cases.racon_layers) on the host into a
+window arena, then b200poa_polisher_polish_arena."""
 import numpy as np
+
+from cut_cases import racon_layers
 
 COMP = bytes.maketrans(b"ACGT", b"TGCA")
 
@@ -24,8 +26,11 @@ def _mutate(rng, s: bytes, e: float) -> bytes:
     return bytes(out)
 
 
-def synth_overlap_set(seed: int, contig_lengths=(3100, 0, 2400, 1750, 4000), depth=6, error=0.08, read_len=(600, 1800)):
-    """Columns for api.polish_overlaps.  Contig 1 is empty when its length is 0; a contig may get no overlap."""
+def synth_overlap_set(seed: int, contig_lengths=(3100, 0, 2400, 1750, 4000), depth=6, error=0.08, read_len=(600, 1800),
+                      long_insertions=0.0):
+    """Columns for api.polish_overlaps.  Contig 1 is empty when its length is 0; a contig may get no overlap.
+    long_insertions: the share of reads with 1100 random bases inserted in their middle, which gives the window
+    there a layer longer than the POA batch's max_sequence_size (1023)."""
     rng = np.random.default_rng(seed)
     contigs = [rng.choice(np.frombuffer(b"ACGT", np.uint8), size=n).tobytes() for n in contig_lengths]
     t_qual = [bytes(rng.integers(33 + 5, 33 + 40, size=len(c), dtype=np.uint8)) for c in contigs]
@@ -38,6 +43,9 @@ def synth_overlap_set(seed: int, contig_lengths=(3100, 0, 2400, 1750, 4000), dep
             tb = int(rng.integers(0, max(1, len(t) - 200)))
             te = min(len(t), tb + ln)
             seg = _mutate(rng, t[tb:te], error)
+            if rng.random() < long_insertions:
+                mid = len(seg) // 2
+                seg = seg[:mid] + bytes(rng.choice(np.frombuffer(b"ACGT", np.uint8), size=1100)) + seg[mid:]
             lead, tail = bytes(rng.choice(np.frombuffer(b"ACGT", np.uint8), size=int(rng.integers(0, 60)))), b""
             strand = int(rng.integers(2))
             has_q = bool(rng.random() < 0.7)
@@ -96,20 +104,12 @@ def host_windows(s, w: int, threshold: float, with_t_qual=True, device=0):
             bb = contig[j:j + w]
             q = s["t_qual"][s["t_off"][c] + j:s["t_off"][c] + j + len(bb)].tobytes() if with_t_qual else b"!" * len(bb)
             arena.add_window(bb, q)
-    for o, bp in zip(ov, bps):
-        for j in range(0, bp.shape[0], 2):
-            (t0, q0), (t1, q1) = (int(x) for x in bp[j]), (int(x) for x in bp[j + 1])
-            if q1 - q0 < 0.02 * w:
-                continue
-            if o["qual"] is not None:
-                avg = 0.0
-                for ch in o["qual"][q0 - o["q_first"]:q1 - o["q_first"]]:
-                    avg += ch - 33
-                if avg / (q1 - q0) < threshold:
-                    continue
-            start = (t0 // w) * w
-            data = o["q"][q0 - o["q_first"]:q1 - o["q_first"]]
-            qq = o["qual"][q0 - o["q_first"]:q1 - o["q_first"]] if o["qual"] is not None else None
-            arena.add_layer(first_window[o["t_id"]] + t0 // w, data, qq, t0 - start, t1 - start - 1)
+    for win, layers in sorted(racon_layers([dict(o, first_window=first_window[o["t_id"]]) for o in ov], bps, w,
+                                           threshold).items()):
+        for k, q0, ln, bg, en, has_q in layers:
+            o = ov[k]
+            data = o["q"][q0 - o["q_first"]:q0 - o["q_first"] + ln]
+            qq = o["qual"][q0 - o["q_first"]:q0 - o["q_first"] + ln] if has_q else None
+            assert arena.add_layer(win, data, qq, bg, en)
     arena.finalize(view=False)
     return arena

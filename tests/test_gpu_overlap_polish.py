@@ -14,11 +14,17 @@ pytestmark = pytest.mark.gpu
 W, THR, SCORES = 500, 10.0, {"match": 5, "mismatch": -4, "gap": -8}
 
 
-@pytest.mark.parametrize("seed", [11, 12])
+#: seed -> the set's arguments.  Seed 14 is deep: windows of more than 200 layers and layers longer than 1023 bases
+#: (reads with long insertions), so the driver's dropped-layer branch and its status choice run.
+SETS = {11: {}, 12: {}, 14: dict(contig_lengths=(1600, 0, 1200), depth=170, long_insertions=0.03)}
+
+
+@pytest.mark.parametrize("seed", list(SETS))
 @pytest.mark.parametrize("with_t_qual", [True, False])
 def test_device_path_equals_host_path(seed, with_t_qual):
     from racon_gpu_b200 import api
-    s = synth_overlap_set(seed)
+    deep = bool(SETS[seed])
+    s = synth_overlap_set(seed, **SETS[seed])
     arena = host_windows(s, W, THR, with_t_qual=with_t_qual)
     pol = api.Polisher(devices=[0], batches_per_device=1, mem_per_batch=2 << 30, **SCORES)
     hc, hl, hp, hs = pol.polish_arena(arena, stride=4096)
@@ -26,17 +32,24 @@ def test_device_path_equals_host_path(seed, with_t_qual):
     want = api.consensus_list(hc, hl)
     n_win = arena.n_windows
     arena.close()
-    assert hp.sum() > n_win // 2 and (~hp).sum() > 0  # polished windows, and backbones (contig without overlaps)
+    if deep:  # windows dropped for depth and for length, and polished ones
+        assert (hs == api.EXCEEDED_MAXIMUM_SEQUENCES_PER_POA).any() and (hs == api.EXCEEDED_MAXIMUM_SEQUENCE_SIZE).any()
+        assert hp.sum() > 0
+    else:
+        assert hp.sum() > n_win // 2 and (~hp).sum() > 0  # polished windows, and backbones (contig without overlaps)
     rounds = set()
     # one round; several rounds (a small aligner batch); several fills of two POA batches from one aligner batch
-    for aligner_mem, batches, per_batch in ((0, 1, 0), (4 << 20, 2, 3), (5 << 20, 2, 1), (6 << 20, 1, 2)):
+    configs = ((0, 1, 0), (4 << 20, 2, 3), (5 << 20, 2, 1), (6 << 20, 1, 2))
+    if deep:  # its contigs do not fit the small aligner batches: one round, POA batches filled once and in several
+        configs = ((0, 1, 0), (0, 2, 3))
+    for aligner_mem, batches, per_batch in configs:
         got, gp, gs, info = api.polish_overlaps(**polish_args(s, with_t_qual), window_length=W, quality_threshold=THR,
                                                 aligner_mem=aligner_mem, poa_batches=batches,
                                                 mem_per_poa_batch=1 << 30, max_windows_per_batch=per_batch, **SCORES)
         assert len(got) == n_win
         assert got == want and (gp == hp).all() and (gs == hs).all(), (aligner_mem, batches, per_batch)
         rounds.add(info["rounds"])
-    assert min(rounds) == 1 and max(rounds) >= 2, rounds
+    assert min(rounds) == 1 and (deep or max(rounds) >= 2), rounds
 
 
 def test_contig_too_large_for_the_aligner_batch_is_reported():

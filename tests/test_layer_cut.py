@@ -9,6 +9,7 @@ import numpy as np
 import pytest
 
 from common import lambda_fixture, overlap_fixture
+from cut_cases import racon_layers
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
@@ -23,6 +24,7 @@ def emu(tmp_path_factory):
                     os.path.join(HERE, "emu", "emu_cut.cpp")], check=True)
     lib = C.CDLL(str(so))
     lib.emu_layer_cut.restype = C.c_int64
+    lib.emu_cut_scan.restype = None
     assert lib.emu_cut_layer_bytes() == LAYER.itemsize
     return lib
 
@@ -100,32 +102,6 @@ def test_cut_reproduces_racon_lambda_windows(emu, case, seed):
         assert rec.shape[0] < run_cut(emu, ov, 500, -1.0, b.n_windows)[0].shape[0]
 
 
-def racon_layers(ov, w, threshold):
-    """src/polisher.cpp:403-457 restated: per window id, the (overlap, q0, length, begin, end, has_q) add_layer gets,
-    in add order.  Window::add_layer's own empty-span check (src/window.cpp:45-47) included."""
-    out = {}
-    for k, o in enumerate(ov):
-        bp = o["bp"]
-        for j in range(0, bp.shape[0], 2):
-            (t0, q0), (t1, q1) = (int(x) for x in bp[j]), (int(x) for x in bp[j + 1])
-            if q1 - q0 < 0.02 * w:
-                continue
-            if o["qual"] is not None:
-                seg = o["qual"][q0 - o["q_first"]:q1 - o["q_first"]]
-                avg = 0.0
-                for c in seg:
-                    avg += c - 33
-                avg /= q1 - q0
-                if avg < threshold:
-                    continue
-            start = (t0 // w) * w
-            if t0 - start == t1 - start - 1:
-                continue
-            out.setdefault(o["first_window"] + t0 // w, []).append((k, q0, q1 - q0, t0 - start, t1 - start - 1,
-                                                                     o["qual"] is not None))
-    return out
-
-
 def synth_overlaps(rng, w, threshold):
     """Overlaps on three contigs with breaking points racon could form: each touches consecutive windows of its contig
     and covers each with one aligned stretch.  Planted edges: a layer of exactly 0.02 * w bases, one just below; a mean
@@ -182,7 +158,7 @@ def test_cut_matches_racon_restatement(emu, seed):
     w, thr = 500, 10.0
     rng = np.random.default_rng(seed)
     ov, n_win = synth_overlaps(rng, w, thr)
-    want = racon_layers(ov, w, thr)
+    want = racon_layers(ov, [o["bp"] for o in ov], w, thr)
     rec, counts, _, _ = run_cut(emu, ov, w, thr, n_win, seed=seed)
     got = {}
     q_off = np.concatenate([[0], np.cumsum([len(o["q"]) for o in ov])[:-1]])
@@ -202,6 +178,20 @@ def test_cut_matches_racon_restatement(emu, seed):
     assert any(not x[5] for v in want.values() for x in v)  # reads without qualities
     # the short last windows of contigs 1 and 3 (230 and 499 bases)
     assert 3 in want and max(x[4] for x in want[3]) < 230 and 9 in want and max(x[4] for x in want[9]) < 499
+
+
+@pytest.mark.parametrize("n_win", [0, 1, 1023, 1024, 1025, 2049, 10000])
+def test_cut_scan_matches_cumsum(emu, n_win):
+    """Phase 2 (aln_cut_scan_kernel's body, run for its 1024 threads): every window's offset is the exclusive prefix
+    sum of the counts, and win_off[n_win] their total, also where a thread owns more than one window (n_win > 1024)
+    and where the last threads own none."""
+    rng = np.random.default_rng(n_win)
+    counts = rng.integers(0, 300, size=max(n_win, 1)).astype(np.int32)[:n_win]
+    counts[rng.random(n_win) < 0.3] = 0  # empty windows between kept ones
+    win_off = np.full(n_win + 1, -7, dtype=np.int64)
+    emu.emu_cut_scan(_p(np.ascontiguousarray(counts), C.c_int32), C.c_int64(n_win), _p(win_off, C.c_int64))
+    want = np.concatenate([[0], np.cumsum(counts, dtype=np.int64)])
+    assert (win_off == want).all(), int(np.flatnonzero(win_off != want)[0])
 
 
 @pytest.mark.parametrize("header,name,fields", [("b200aln.h", "b200aln_layer", ["overlap", "window", "begin"]),
