@@ -27,6 +27,7 @@
  *                                   src/polisher.cpp:384-457, src/cuda/cudapolisher.cpp:216-345
  *   b200poa_polish_overlaps_ex   <- the same, plus the windows racon's GPU limits leave to its CPU pass
  *                                   (cudapolisher.cpp:354-383): polished on the device, or handed back
+ *   b200poa_polish_overlaps_multi <- the same on every device, contigs too large for one aligner batch split
  *
  * Plain C types only: no C++ objects, no exceptions, no torch types cross this boundary.
  * Status codes are the values of cudapoa::StatusType (cudapoa.hpp:32-45) plus three extensions.
@@ -173,7 +174,8 @@ int32_t b200poa_batch_add_windows_from_aligner(b200poa_batch* b, const struct b2
  * offsets of q_qual where has_quality[k] (reverse_quality() for '-').  Outputs per window, contig by contig
  * (id_to_first_window_id order): those of b200poa_polisher_polish.  *n_rounds: aligner rounds; h2d / d2h_bytes: PCIe
  * bytes of every batch.  A contig whose overlaps do not fit one aligner batch (aligner_mem) is not split:
- * B200POA_GENERIC_ERROR with *unfit_contig = its index (-1 otherwise).
+ * B200POA_GENERIC_ERROR with *unfit_contig = its index (-1 otherwise).  b200poa_polish_overlaps_multi runs the same on
+ * several devices and splits such a contig.
  */
 typedef struct b200poa_overlap_options {
     int32_t device_id;
@@ -243,6 +245,37 @@ int32_t b200poa_polish_overlaps_ex(const b200poa_overlap_options* opt, b200poa_o
                                    int64_t* h2d_bytes, int64_t* d2h_bytes, int64_t* unfit_contig);
 /* frees the arrays of an export and zeroes it */
 void b200poa_free_export(b200poa_overlap_export* e);
+
+/*
+ * b200poa_polish_overlaps_ex on several devices, with contigs too large for one aligner batch split at window boundaries
+ * (racon_b200::polish_overlaps with a device list, overlap_polisher.hpp).  One worker -- an aligner batch, `poa_batches`
+ * POA batches and, with deep_windows, a second-tier batch, on a host thread of its own -- per entry of device_ids; a
+ * device listed twice runs two workers.  n_devices == 0: one worker on every visible device.  opt->device_id is ignored.
+ * mem_per_poa_batch 0: 0.9 * the device's free memory / (workers on it * (poa_batches + 1 + deep_windows)), read once per
+ * device before any worker allocates.
+ * The work is planned up front in units: runs of whole contigs, as b200poa_polish_overlaps's rounds, and for a contig
+ * whose overlaps do not fit one aligner batch alone, consecutive window ranges, each with the overlaps whose window span
+ * meets it (in racon's order), each as long as fits.  Every window gets the same layers in the same order as in a
+ * whole-contig round.  Every worker gets the smallest device's memory share, and with aligner_mem 0 every unit is
+ * planned for it.  A second-tier window is polished exactly when the largest second-tier batch that share allows
+ * polishes it (it climbs the sizes from its own in steps of 512), so the outputs and the export (byte for byte,
+ * ascending window id) do not depend on the number of workers, which worker ran which unit, or where a contig was
+ * split.  They equal b200poa_polish_overlaps_ex's, except that a window its round-sized second tier leaves unpolished
+ * for a graph or consensus limit may be polished here.
+ * ex: nullable (both options off).  *n_rounds: units; *split_contigs: contigs polished in more than one unit;
+ * *repeat_overlaps: alignments done more than once because of the splits (an overlap crossing a unit boundary is aligned
+ * in every unit it meets).  B200POA_INVALID_ARGUMENT for a device id out of range, before anything is allocated;
+ * B200POA_GENERIC_ERROR with *unfit_contig set when the overlaps of one window alone do not fit one aligner batch.
+ */
+int32_t b200poa_polish_overlaps_multi(const b200poa_overlap_options* opt, b200poa_overlap_ex* ex, int32_t n_devices,
+                                      const int32_t* device_ids, int64_t n_contigs, const uint8_t* t_bases,
+                                      const int64_t* t_off, const uint8_t* t_qual, int64_t n_overlaps, const int32_t* t_id,
+                                      const int32_t* t_begin, const int32_t* t_end, const uint8_t* q_bases,
+                                      const int64_t* q_off, const uint8_t* q_qual, const uint8_t* has_quality,
+                                      const int32_t* q_first, uint8_t* cons_out, int32_t stride, int32_t* cons_len,
+                                      uint8_t* polished, int32_t* status_out, int64_t* n_rounds, int64_t* h2d_bytes,
+                                      int64_t* d2h_bytes, int64_t* unfit_contig, int64_t* split_contigs,
+                                      int64_t* repeat_overlaps);
 
 void b200poa_weight_modes(int64_t n_sequences, const int64_t* seq_off, const int8_t* weights,
                           const uint8_t* has_weights, int64_t* weight_mode);

@@ -47,7 +47,7 @@ ABI_SYMBOLS = (
     "b200poa_arena_create", "b200poa_arena_add_window", "b200poa_arena_add_layer", "b200poa_arena_finalize",
     "b200poa_arena_view", "b200poa_polisher_polish_arena", "b200poa_arena_destroy",
     "b200poa_batch_add_windows_from_aligner", "b200poa_polish_overlaps", "b200poa_polish_overlaps_ex",
-    "b200poa_free_export",
+    "b200poa_free_export", "b200poa_polish_overlaps_multi",
 )
 
 
@@ -648,7 +648,7 @@ def polish_overlaps(t_bases, t_off, t_qual, t_id, t_begin, t_end, q_bases, q_off
                     window_length=500, quality_threshold=10.0, match=3, mismatch=-5, gap=-4, banded=False, tgs=True,
                     trim=True, device=0, poa_batches=1, mem_per_poa_batch=0, aligner_mem=0, max_windows_per_batch=0,
                     stride=4096, deep_windows=False, export_layers=False, deep_max_sequence_size=0,
-                    deep_max_sequences_per_poa=0):
+                    deep_max_sequences_per_poa=0, devices=None):
     """b200poa_polish_overlaps (racon_b200::polish_overlaps): contigs and racon's filtered overlaps in, per window
     (contig by contig) the consensus list, polished, status out, plus {"rounds", "h2d_bytes", "d2h_bytes"}.
     Raises when a contig's overlaps do not fit one aligner batch (the error names the contig).
@@ -657,7 +657,13 @@ def polish_overlaps(t_bases, t_off, t_qual, t_id, t_begin, t_end, q_bases, q_off
     unpolished (b200poa_polish_overlaps_ex; deep_max_* cap that tier, 0 = the engine's limits).  export_layers: the
     windows still unpolished with at least 3 sequences come back as info["export"] = (window ids, WindowBatch in the
     layout of racon_gpu_b200/windows.py), ready for Polisher.polish or racon's CPU pass.  With either set, info also
-    has "tier2_windows", "tier2_polished", "tier2_batches", "exported_windows" and "exported_bytes"."""
+    has "tier2_windows", "tier2_polished", "tier2_batches", "exported_windows" and "exported_bytes".
+
+    devices: None runs on `device` alone, as above.  A list runs one worker per entry (b200poa_polish_overlaps_multi;
+    [] = every visible device, an id listed twice = two workers on it) and splits a contig too large for one aligner
+    batch at window boundaries; the outputs equal the single-device call's.  info["rounds"] then counts units, and info
+    also has "split_contigs" (contigs polished in more than one unit) and "repeat_overlaps" (alignments done more than
+    once because of the splits)."""
     lib = load_library()
     o = OverlapOptions(device, poa_batches, mem_per_poa_batch, aligner_mem, window_length, float(quality_threshold),
                        int(bool(banded)), match, mismatch, gap, int(tgs), int(trim), max_windows_per_batch)
@@ -673,6 +679,7 @@ def polish_overlaps(t_bases, t_off, t_qual, t_id, t_begin, t_end, q_bases, q_off
     pol = np.zeros(max(n_win, 1), dtype=np.uint8)
     st = np.zeros(max(n_win, 1), dtype=np.int32)
     rounds, h2d, d2h, unfit = C.c_int64(0), C.c_int64(0), C.c_int64(0), C.c_int64(-1)
+    split, repeat = C.c_int64(0), C.c_int64(0)
     u8 = lambda a: None if a is None else _p(np.ascontiguousarray(a, dtype=np.uint8), C.c_uint8)
     keep = [np.ascontiguousarray(a, dtype=d) for a, d in ((t_bases, np.uint8), (q_bases, np.uint8),
                                                            (t_id, np.int32), (t_begin, np.int32), (t_end, np.int32),
@@ -685,7 +692,16 @@ def polish_overlaps(t_bases, t_off, t_qual, t_id, t_begin, t_end, q_bases, q_off
             _p(keep[1], C.c_uint8), _p(keep[5], C.c_int64), u8(qq), u8(hq), _p(keep[6], C.c_int32),
             _p(cons, C.c_uint8), C.c_int32(stride), _p(clen, C.c_int32), _p(pol, C.c_uint8), _p(st, C.c_int32),
             C.byref(rounds), C.byref(h2d), C.byref(d2h), C.byref(unfit))
-    if ex is None:
+    if devices is not None:
+        dev = np.ascontiguousarray(list(devices), dtype=np.int32)
+        lib.b200poa_free_export.restype = None
+        rc = lib.b200poa_polish_overlaps_multi(C.byref(o), None if ex is None else C.byref(ex), C.c_int32(len(dev)),
+                                               _p(dev, C.c_int32) if len(dev) else None, *args, C.byref(split),
+                                               C.byref(repeat))
+        if ex is not None:
+            exported = _export_batch(ex.exported) if rc == SUCCESS and export_layers else None
+            lib.b200poa_free_export(C.byref(ex.exported))
+    elif ex is None:
         rc = lib.b200poa_polish_overlaps(C.byref(o), *args)
     else:
         lib.b200poa_free_export.restype = None
@@ -694,9 +710,13 @@ def polish_overlaps(t_bases, t_off, t_qual, t_id, t_begin, t_end, q_bases, q_off
         lib.b200poa_free_export(C.byref(ex.exported))
     if rc != SUCCESS:
         what = f" (contig {unfit.value} does not fit one aligner batch)" if unfit.value >= 0 else ""
+        if devices is not None and unfit.value >= 0:
+            what = f" (the overlaps of one window of contig {unfit.value} do not fit one aligner batch)"
         raise RuntimeError(f"b200poa_polish_overlaps failed: {status_string(rc)}{what}")
     out = [cons[i, :min(int(clen[i]), stride)].tobytes() for i in range(n_win)]
     info = {"rounds": int(rounds.value), "h2d_bytes": int(h2d.value), "d2h_bytes": int(d2h.value)}
+    if devices is not None:
+        info.update({"split_contigs": int(split.value), "repeat_overlaps": int(repeat.value)})
     if ex is not None:
         info.update({k: int(getattr(ex, k)) for k in ("tier2_windows", "tier2_polished", "tier2_batches",
                                                        "exported_windows", "exported_bytes")})

@@ -15,7 +15,8 @@ LIB = os.path.join(HERE, "libb200poa.so")
 SOURCES = ["b200poa.cu", "b200aln.cu", "host/cuda_batch.cpp", "host/cuda_polisher.cpp", "host/overlap_polisher.cpp"]
 HEADERS = ["poa_core.cuh", "poa_fill.cuh", "poa_simt.cuh", "cuda_buffers.hpp", "host/b200_window.hpp", "host/cuda_batch.hpp",
            "host/cuda_polisher.hpp", "host/overlap_polisher.hpp", "host/b200poa_batch.hpp", "host/window_arena.hpp", "../../include/b200poa.h",
-           "aln_core.cuh", "layer_cut.cuh", "host/aln_levels.hpp", "host/b200aln_aligner.hpp", "../../include/b200aln.h"]
+           "aln_core.cuh", "aln_layout.cuh", "layer_cut.cuh", "host/aln_levels.hpp", "host/aln_admission.hpp",
+           "host/overlap_units.hpp", "host/b200aln_aligner.hpp", "../../include/b200aln.h"]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",

@@ -34,6 +34,7 @@
 #include "../../include/b200aln.h"
 #include "aln_core.cuh"
 #include "cuda_buffers.hpp"
+#include "host/aln_admission.hpp"
 #include "host/aln_levels.hpp"
 #include "layer_cut.cuh"
 
@@ -45,21 +46,6 @@ static_assert(sizeof(CutLayer) == sizeof(b200aln_layer) && offsetof(CutLayer, wi
               "the layer records leave the device as they are");
 
 namespace {
-
-struct AlnJob { /* one alignment of the batch */
-    int64_t q_off, t_off; /* into the sequence arena */
-    int64_t ops_off;      /* into the operations arena (n + m bytes) */
-    int32_t n, m;
-    int32_t q_first, t_begin; /* where the segments start in read / contig coordinates (breaking points only) */
-};
-struct AlnResult {
-    int32_t score, status, n_runs, n_ops;
-    int64_t runs_off;  /* into the runs arena (words)  */
-    int64_t cigar_off; /* into the text arena (bytes)  */
-    int32_t cigar_len; /* without the terminating 0    */
-    int32_t bp_count;  /* breaking points ((t, q) pairs) */
-    int64_t bp_off;    /* into the breaking-point arena (pairs) */
-};
 
 enum { /* int32 words of the device counter block */
     CT_CURSOR = 0,      /* [128] one work cursor per launch                                  */
@@ -96,8 +82,6 @@ struct AlnKernelArgs {
     int32_t leaf_log_cap;
 #endif
 };
-
-constexpr int WARPS_PER_BLOCK = 2;
 
 /* what one split launch works through: up to three lists of a level, one after the other (largest shapes first) */
 struct AlnWork {
@@ -468,8 +452,7 @@ struct b200aln_batch {
     std::vector<AlnJob> jobs;
     int64_t ops_bytes = 0;
     int64_t cap_open = 0, cap_leaves = 0; /* list capacities the staged alignments need */
-    int32_t max_len = 0;
-    int64_t var_bytes = 0; /* device bytes the staged alignments need besides the slots */
+    AlnLoad load; /* what the staged alignments hold of the budget (host/aln_admission.hpp) */
 
     /* device */
     DevBuf d_slab, d_team_slab, d_seq, d_jobs, d_ops, d_res, d_runs, d_text, d_bp, d_list[ALN_CLASSES][2], d_leaves, d_counters;
@@ -532,30 +515,12 @@ namespace {
         }                                          \
     } while (0)
 
-int64_t slot_bytes_for(int32_t max_len) {
-    size_t total = 0;
-    AlnSlot s;
-    aln_slot_bind(s, nullptr, max_len, &total);
-    return (int64_t)total;
-}
-int32_t round_len(int32_t len) { /* slots are re-made only when the longest sequence outgrows them */
-    int32_t r = 16384;
-    while (r < len + 1 && r < (1 << 30)) r <<= 1;
-    return r;
-}
-/* device bytes one alignment needs besides the slots: sequences, operations, run starts, its share of the lists */
-int64_t var_bytes_for(int32_t n, int32_t m) {
-    const int64_t len = (int64_t)n + m;
-    return 8 * len + 80 + (int64_t)sizeof(AlnJob) + (int64_t)sizeof(AlnResult) +
-           (2 * aln_open_capacity(n, m) + aln_leaf_capacity(n, m)) * (int64_t)sizeof(AlnRect);
-}
-
 int32_t ensure_slots(b200aln_batch* b) {
-    const int32_t want_len = round_len(b->max_len);
+    const int32_t want_len = round_len(b->load.max_len);
     if (b->n_slots > 0 && want_len <= b->slot_max_len) return B200ALN_SUCCESS;
     const int64_t sb = slot_bytes_for(want_len);
     const int64_t resident = (int64_t)b->sm_count * b->blocks_per_sm * WARPS_PER_BLOCK;
-    int64_t avail = b->budget - b->var_bytes;
+    int64_t avail = b->budget - b->load.var_bytes;
     /* team workspaces (tall sub-problems of thin levels) take at most a quarter of what is left; none is fine too:
      * tall sub-problems then run one warp each */
     size_t tsb = 0;
@@ -771,11 +736,6 @@ int32_t b200aln_batch_add_alignment(b200aln_batch* b, const char* query, int32_t
     return b200aln_batch_add_overlap(b, query, n, target, m, 0, 0);
 }
 
-/* device bytes the layer cut adds per overlap: the quality arena (it mirrors the whole sequence arena, so that a layer's
- * qualities sit at its bases' offset), and per window it touches its item, place and record */
-static int64_t cut_bytes_for(const b200aln_batch* b, int32_t n, int32_t m, int64_t n_win) {
-    return b->layer_cut ? (int64_t)n + m + (2 * (int64_t)sizeof(CutLayer) + 8) * n_win : 0;
-}
 /* the layer cut's inputs of one overlap are admissible (b200aln_layer_inputs) */
 static bool cut_inputs_ok(int32_t m, int32_t t_begin, int64_t first_window, int32_t t_length) {
     return first_window >= 0 && first_window < ((int64_t)1 << 31) - ((int64_t)t_length + 1) && (int64_t)t_begin + m <= t_length;
@@ -789,15 +749,9 @@ static int32_t add_one(b200aln_batch* b, const char* query, int32_t n, const cha
     if ((int64_t)t_begin + m >= ((int64_t)1 << 31) || (int64_t)q_first + n >= ((int64_t)1 << 31)) return B200ALN_INVALID_ARGUMENT;
     if (b->layer_cut && !cut_inputs_ok(m, t_begin, first_window, t_length)) return B200ALN_INVALID_ARGUMENT;
     if (b->aligned || b->view_q) return B200ALN_GENERIC_ERROR; /* reset() first, like a cudaaligner batch after align_all */
-    if ((int64_t)n + m >= ((int64_t)1 << 30)) return B200ALN_EXCEEDED_MAX_LENGTH; /* run starts are 30-bit */
-    const int64_t n_win = aln_window_count(t_begin, m, b->window_length);
-    const int64_t vb = var_bytes_for(n, m) + 16 * n_win + cut_bytes_for(b, n, m, n_win);
-    const int32_t new_max = std::max(b->max_len, std::max(n, m));
-    /* the slots get what the alignments leave; at least one block's worth must remain */
-    const int64_t min_slots = WARPS_PER_BLOCK * slot_bytes_for(round_len(new_max));
-    if (vb + min_slots > b->budget) return B200ALN_EXCEEDED_MAX_LENGTH;
-    if (b->var_bytes + vb + min_slots > b->budget) return B200ALN_EXCEEDED_MAX_ALIGNMENTS;
-    if (b->jobs.size() >= (size_t)0x7FFFFF00) return B200ALN_EXCEEDED_MAX_ALIGNMENTS;
+    AlnLoad load = b->load;
+    const int32_t adm = aln_admit(load, b->budget, b->window_length, b->layer_cut, n, m, t_begin);
+    if (adm != B200ALN_SUCCESS) return adm;
     if (b->h_seq.used + (size_t)n + (size_t)m > b->h_seq.cap) cudaSetDevice(b->device); /* the staging buffer grows: page-lock it in this batch's context */
     if (!b->h_seq.reserve(b->h_seq.used + (size_t)n + (size_t)m)) return B200ALN_GENERIC_ERROR;
     if (b->layer_cut) { /* the qualities take the query's offsets in a buffer of their own */
@@ -823,12 +777,11 @@ static int32_t add_one(b200aln_batch* b, const char* query, int32_t n, const cha
     j.m = m;
     j.q_first = q_first;
     j.t_begin = t_begin;
-    b->n_windows += n_win;
+    b->n_windows += aln_window_count(t_begin, m, b->window_length);
     b->ops_bytes += (int64_t)n + m;
     b->cap_open += aln_open_capacity(n, m);
     b->cap_leaves += aln_leaf_capacity(n, m);
-    b->var_bytes += vb;
-    b->max_len = new_max;
+    b->load = load;
     b->jobs.push_back(j);
     return B200ALN_SUCCESS;
 }
@@ -1350,12 +1303,8 @@ int32_t b200aln_batch_add_overlaps_view_ex(b200aln_batch* b, int64_t n, const ui
         int32_t tl = 0;
         layer_inputs_of(li, q_off, k, tb, mi, &qual, &fw, &tl);
         if (b->layer_cut && !cut_inputs_ok(mi, tb, fw, tl)) { st = B200ALN_INVALID_ARGUMENT; break; }
-        const int64_t n_win = aln_window_count(tb, mi, b->window_length);
-        const int64_t vb = var_bytes_for(ni, mi) + 16 * n_win + cut_bytes_for(b, ni, mi, n_win);
-        const int32_t new_max = std::max(b->max_len, std::max(ni, mi));
-        const int64_t min_slots = WARPS_PER_BLOCK * slot_bytes_for(round_len(new_max));
-        if (vb + min_slots > b->budget) { st = B200ALN_EXCEEDED_MAX_LENGTH; break; }
-        if (b->var_bytes + vb + min_slots > b->budget || b->jobs.size() >= (size_t)0x7FFFFF00) { st = B200ALN_EXCEEDED_MAX_ALIGNMENTS; break; }
+        st = aln_admit(b->load, b->budget, b->window_length, b->layer_cut, ni, mi, tb);
+        if (st != B200ALN_SUCCESS) break;
         if (b->layer_cut) {
             b->cut_first_window.push_back(fw);
             b->cut_t_length.push_back(tl);
@@ -1369,12 +1318,10 @@ int32_t b200aln_batch_add_overlaps_view_ex(b200aln_batch* b, int64_t n, const ui
         j.m = mi;
         j.q_first = qf;
         j.t_begin = tb;
-        b->n_windows += n_win;
+        b->n_windows += aln_window_count(tb, mi, b->window_length);
         b->ops_bytes += nn + mm;
         b->cap_open += aln_open_capacity(ni, mi);
         b->cap_leaves += aln_leaf_capacity(ni, mi);
-        b->var_bytes += vb;
-        b->max_len = new_max;
         b->jobs.push_back(j);
     }
     if (k > 0) {
@@ -1494,8 +1441,7 @@ int32_t b200aln_batch_reset(b200aln_batch* b) {
     b->n_windows = 0;
     b->h_bp.used = 0;
     b->cap_open = b->cap_leaves = 0;
-    b->var_bytes = 0;
-    b->max_len = 0;
+    b->load = AlnLoad{};
     b->res.clear();
     b->h_runs.used = 0;
     b->h_text.used = 0;

@@ -1,7 +1,7 @@
 /*
  * aln_levels.hpp -- host-side helpers of the level-synchronous Hirschberg recursion (aln_core.cuh) shared by the batch
- * runtime (csrc/b200aln.cu) and the lane emulation (tests/emu/emu_aln.cpp): capacity of the sub-problem lists, and the
- * expansion of run starts (aln_runs) into operations / a CIGAR string.
+ * runtime (csrc/b200aln.cu) and the lane emulation (tests/emu/emu_aln.cpp): the expansion of run starts (aln_runs) into
+ * operations / a CIGAR string.  The capacity of the sub-problem lists is in aln_layout.cuh.
  */
 #pragma once
 #include <cstdint>
@@ -11,15 +11,6 @@
 #include "../aln_core.cuh"
 
 namespace b200aln {
-
-/* How many sub-problems one n x m alignment can have open at one level / leave as leaves in total.  A split halves the
- * columns and partitions the rows, so level d holds <= min(2^d, data / 2^d / 1 MB + 1) open sub-problems (each open one
- * carries >= 1 MB of leaf data, edlib.cpp:1155-1157); every open sub-problem has two children. */
-inline int64_t aln_open_capacity(int32_t n, int32_t m) {
-    const int64_t data = 20 * (int64_t)((n + 63) / 64) * m + 8 * (int64_t)m;
-    return 2 * (data / ALN_LEAF_DATA_LIMIT + 1) + 2;
-}
-inline int64_t aln_leaf_capacity(int32_t n, int32_t m) { return 4 * aln_open_capacity(n, m) + 2; }
 
 /* run starts (start << 2 | op) + total operation count -> one operation per position (edlib's EDLIB_EDOP_* codes) */
 inline void aln_expand_runs(const uint32_t* runs, int32_t n_runs, int32_t n_ops, std::vector<uint8_t>& out) {

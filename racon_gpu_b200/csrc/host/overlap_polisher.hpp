@@ -1,21 +1,30 @@
 /*
- * overlap_polisher.hpp -- polish contigs from aligned overlaps on one device without the host window arena:
+ * overlap_polisher.hpp -- polish contigs from aligned overlaps on the device without the host window arena:
  * the loop at the end of racon's Polisher::initialize (src/polisher.cpp:400-457) and the GPU section of
- * CUDAPolisher::polish (src/cuda/cudapolisher.cpp:216-345) for one device.
+ * CUDAPolisher::polish (src/cuda/cudapolisher.cpp:216-345), on one device or on several.
  *
- * The work runs in rounds of WHOLE contigs: a window only receives layers from overlaps on its own contig, so a round is
- * a run of consecutive contigs together with all their overlaps (a stable partition of racon's overlap order by t_id).
- * One aligner batch per round aligns them, forms the breaking points and cuts the layers on the device
- * (b200aln_batch_set_layer_cut); the device's POA batches then gather the layers from the aligner's arena
- * (b200poa_batch_add_windows_from_aligner) until every window of the round is polished, and only then is the aligner
- * batch reset.  A contig whose overlaps do not fit one aligner batch is reported (unfit_contig), never split.
+ * The work runs in UNITS (overlap_units.hpp), planned from the input before any batch exists: runs of whole contigs, and
+ * with a device list, window ranges of a contig too large for one aligner batch.  A window only receives layers from
+ * overlaps on its own contig, so a unit is a run of windows together with every overlap whose window span meets it, in
+ * racon's order.  One aligner batch per unit aligns them, forms the breaking points and cuts the layers on the device
+ * (b200aln_batch_set_layer_cut); the device's POA batches then gather the layers of the windows the unit owns from the
+ * aligner's arena (b200poa_batch_add_windows_from_aligner), and only then is the aligner batch reset.  Without a device
+ * list a contig whose overlaps do not fit one aligner batch is reported (unfit_contig), never split.
+ *
+ * Each WORKER -- one per entry of the device list, so a device listed twice runs two -- owns an aligner batch,
+ * `poa_batches` POA batches, an optional second-tier batch and their streams, on a host thread of its own.  Workers
+ * claim units from one cursor and write the rows of the windows they own directly; the export is merged in unit order,
+ * which is ascending window id.  Units depend on the input and the aligner budget only; every worker gets the smallest
+ * device's memory share; and each second-tier window climbs the batch sizes from its own until it is polished or no
+ * larger batch fits that share (polish_unit), so the outputs do not depend on how many workers ran the units, which
+ * one took which unit, or where a contig was split.
  *
  * The POA batches have racon's GPU limits (1023 bases per sequence, 200 sequences per window, cudabatch.cpp:56-59).  With
  * deep_windows, a second tier takes the windows they cannot take whole -- more than 200 sequences, or one longer than
- * 1023 bases -- in one more POA batch sized from the round's records (b200aln_batch_get_layers): its
+ * 1023 bases -- in one more POA batch per worker sized from the unit's records (b200aln_batch_get_layers): its
  * max_sequences_per_poa the deepest such window's sequence count, its max_sequence_size their longest sequence rounded
- * up to a multiple of 512 less one.  That batch lives across rounds and is re-created only when a round needs larger
- * limits.  With export_layers, every window still unpolished after both tiers that has at least 3 sequences comes back
+ * up to a multiple of 512 less one.  That batch lives across units and is re-created only when a unit needs larger
+ * limits (with a device list: also when a window climbs to a larger size).  With export_layers, every window still unpolished after both tiers that has at least 3 sequences comes back
  * as a host window arena (b200aln_batch_export_layers: one kernel and one D2H of exactly its layers' bytes), so that
  * racon's CPU pass can redo it as it does for the windows its GPU path fails (cudapolisher.cpp:354-383).
  * Parsing, overlap filtering (remove_invalid_overlaps), the CPU redo of unpolished windows and stitching stay in racon.
@@ -28,9 +37,9 @@
 namespace racon_b200 {
 
 struct OverlapPolishOptions {
-    int32_t device = 0;
-    int32_t poa_batches = 1;          /* racon -c: POA batches of the device */
-    size_t mem_per_poa_batch = 0;     /* 0 = 0.9 * free / (poa_batches + 1) */
+    int32_t device = 0;               /* the device without a device list */
+    int32_t poa_batches = 1;          /* racon -c: POA batches of a worker */
+    size_t mem_per_poa_batch = 0;     /* 0 = 0.9 * free / (workers on the device * (poa_batches + 1 + deep_windows)) */
     int64_t aligner_mem = 0;          /* 0 = the same share as one POA batch */
     int32_t window_length = 500;      /* racon -w */
     double quality_threshold = 10.0;  /* racon -q */
@@ -85,7 +94,7 @@ struct OverlapPolishOutput {
     int32_t* cons_len;
     uint8_t* polished;
     int32_t* status;
-    int64_t n_rounds = 0;
+    int64_t n_rounds = 0;                 /* units */
     int64_t h2d_bytes = 0, d2h_bytes = 0; /* aligner and POA batches together */
     int64_t unfit_contig = -1;            /* a contig whose overlaps do not fit one aligner batch */
     int64_t tier2_windows = 0;            /* windows given to the second tier */
@@ -94,13 +103,23 @@ struct OverlapPolishOutput {
     int64_t exported_windows = 0;         /* windows appended to *exported */
     int64_t exported_bytes = 0;           /* bytes their export moved device -> host (bases and weights) */
     OverlapExport* exported = nullptr;    /* with export_layers: where the exported windows are appended */
+    int64_t split_contigs = 0;            /* contigs polished in more than one unit */
+    int64_t repeat_overlaps = 0;          /* alignments done more than once because of the splits */
 };
 
 /* The number of windows of the input (sum over contigs of ceil(length / window_length)). */
 int64_t overlap_window_count(const OverlapInput& in, int32_t window_length);
 
-/* Returns a b200poa status: B200POA_SUCCESS, B200POA_INVALID_ARGUMENT, B200POA_CUDA_ERROR, or B200POA_GENERIC_ERROR
- * with out.unfit_contig set when a contig's overlaps do not fit one aligner batch. */
+/* On opt.device, in units of whole contigs.  Returns a b200poa status: B200POA_SUCCESS, B200POA_INVALID_ARGUMENT,
+ * B200POA_CUDA_ERROR, or B200POA_GENERIC_ERROR with out.unfit_contig set when a contig's overlaps do not fit one aligner
+ * batch. */
 int32_t polish_overlaps(const OverlapInput& in, const OverlapPolishOptions& opt, OverlapPolishOutput& out);
+
+/* On one worker per entry of `devices` (empty: every visible device; opt.device is not used), a contig too large for
+ * one aligner batch split at window boundaries.  With aligner_mem 0 every unit is planned for the smallest worker's
+ * share.  B200POA_INVALID_ARGUMENT for a device id out of range, before anything is allocated; B200POA_GENERIC_ERROR
+ * with out.unfit_contig set when the overlaps of one window alone do not fit one aligner batch. */
+int32_t polish_overlaps(const OverlapInput& in, const OverlapPolishOptions& opt, const std::vector<int32_t>& devices,
+                        OverlapPolishOutput& out);
 
 } // namespace racon_b200
